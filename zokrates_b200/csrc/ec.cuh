@@ -4,7 +4,9 @@
 //
 // Accumulators use extended Jacobian "XYZZ" coordinates (x = X/ZZ, y = Y/ZZZ, ZZ^3 = ZZZ^2):
 // mixed addition 8M + 2S (= 10 field multiplications, the SURVEY.md §8d accounting unit), full
-// addition 12M + 2S, doubling 6M + 3S.  Results are representation independent: the affine point
+// addition 12M + 2S, doubling 6M + 3S.  The squarings use the dedicated square (fp.cuh sqr_wide), and
+// Y3 = Rd (Q - X3) - Y1 PPP is F::mul_sub: two wide products summed and reduced once (DESIGN.md §4 gives the
+// resulting multiply-add counts).  Results are representation independent: the affine point
 // is canonical, so outputs are bit-identical to any other correct implementation.
 #pragma once
 #include "fp2.cuh"
@@ -72,7 +74,7 @@ struct XYZZ {
     F PPP = F::mul(Pd, PP);
     F Q = F::mul(a.x, PP);
     F X3 = F::sub(F::sub(F::sqr(Rd), PPP), F::dbl(Q));
-    F Y3 = F::sub(F::mul(Rd, F::sub(Q, X3)), F::mul(a.y, PPP));
+    F Y3 = F::mul_sub(Rd, F::sub(Q, X3), a.y, PPP);  // one reduction for both products
     return XYZZ{X3, Y3, F::mul(a.zz, PP), F::mul(a.zzz, PPP)};
   }
 
@@ -94,7 +96,7 @@ struct XYZZ {
     F PPP = F::mul(Pd, PP);
     F Q = F::mul(U1, PP);
     F X3 = F::sub(F::sub(F::sqr(Rd), PPP), F::dbl(Q));
-    F Y3 = F::sub(F::mul(Rd, F::sub(Q, X3)), F::mul(S1, PPP));
+    F Y3 = F::mul_sub(Rd, F::sub(Q, X3), S1, PPP);
     return XYZZ{X3, Y3, F::mul(F::mul(a.zz, b.zz), PP), F::mul(F::mul(a.zzz, b.zzz), PPP)};
   }
 

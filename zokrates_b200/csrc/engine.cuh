@@ -275,7 +275,10 @@ inline uint32_t msm_pick_c_pre(uint64_t n, int fr_bits, uint64_t max_w = 16 /* m
   for (uint32_t c = 4; c <= 22; c++) {
     uint64_t W = (fr_bits + 1 + c - 1) / c;
     if (W > max_w || n * W >= (1ull << 31)) continue;
-    // 10 multiplications per mixed addition; a bucket costs ~70 in the reductions (segmented partial levels + bit sums)
+    // relative costs in Fq multiplications: 10 per mixed addition, ~70 per bucket in the reductions (segmented partial
+    // levels + bit sums, full additions).  The dedicated square and the once-reduced Y3 (DESIGN.md §4) made both sides
+    // cheaper by similar fractions (G1 mixed addition 1360 -> 1232 wide MADs, -9.4 %; full addition 1904 -> 1776, -6.7 %),
+    // so the 10 : 70 ratio, and with it the window picked at every size, stays as measured on H100 (DESIGN.md §7)
     double cost = (double)W * 10.0 * (double)n + 70.0 * (double)(1u << (c - 1));
     if (cost < best_cost) { best_cost = cost; best = c; }
   }

@@ -72,6 +72,10 @@ struct alignas(16) Fp64 {
     return (t[N] || geq_p(o)) ? sub_p(o) : o;
   }
   ZKB_HD static Fp64 sqr(const Fp64& a) { return mul(a, a); }
+  // the interface Fp2T and XYZZ use; this serial host path reduces every product (no Wide)
+  static constexpr bool LAZY_HEADROOM = false;
+  ZKB_HD static Fp64 add_nr(const Fp64& a, const Fp64& b) { return add(a, b); }
+  ZKB_HD static Fp64 mul_sub(const Fp64& a, const Fp64& b, const Fp64& c, const Fp64& d) { return sub(mul(a, b), mul(c, d)); }
   ZKB_HD static Fp64 mul_ni(const Fp64& a, const Fp64& b) { return mul(a, b); }
   ZKB_HD static Fp64 to_mont(const Fp64& a) { return mul(a, r2()); }
   ZKB_HD static Fp64 from_mont(const Fp64& a) { Fp64 o = zero(); o.v[0] = 1; return mul(a, o); }
