@@ -35,10 +35,11 @@ extern "C" {
 #define ZKB_E_UNSAT 5
 #define ZKB_E_INTERNAL 6
 
-/* curve ids: the curves of BASELINE.json; names as zokrates_field `Field::name()`
- * (zokrates_field/src/bn128.rs:1-13, bls12_381.rs:1-13) */
+/* curve ids: the curves of BASELINE.json and BLS12-377; names as zokrates_field `Field::name()`
+ * (zokrates_field/src/bn128.rs:1-13, bls12_381.rs:1-13, bls12_377.rs:1-13) */
 #define ZKB_CURVE_BN128 0
 #define ZKB_CURVE_BLS12_381 1
+#define ZKB_CURVE_BLS12_377 2
 
 typedef struct zkb_ctx zkb_ctx;
 

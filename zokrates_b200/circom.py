@@ -49,8 +49,19 @@ def r1cs_program(prog: Prog):
     return variables, private_offset, rows
 
 
+# the fields snarkjs / iden3 know; BLS12-377 is not one of them
+CIRCOM_CURVES = ("bn128", "bls12_381")
+
+
+def _circom_curve(curve):
+    c = _curve(curve)
+    if c.name not in CIRCOM_CURVES:
+        raise ValueError("circom export supports bn128 and bls12_381, not %s" % c.name)
+    return c
+
+
 def write_r1cs(prog: Prog) -> bytes:
-    c = _curve(prog.curve)
+    c = _circom_curve(prog.curve)
     n8 = (c.r.bit_length() + 7) // 8
     variables, _, rows = r1cs_program(prog)
     n_pub_in = sum(not p.private for p in prog.arguments)
@@ -92,7 +103,7 @@ def read_r1cs(data: bytes) -> R1CS:
     (n8,) = struct.unpack_from("<I", data, ho)
     prime = int.from_bytes(data[ho + 4:ho + 4 + n8], "little")
     n_wires, n_out, n_pub, n_prv, n_labels, n_cons = struct.unpack_from("<IIIIQI", data, ho + 4 + n8)
-    cv = next((c for c in map(_curve, ("bn128", "bls12_381")) if c.r == prime), None)
+    cv = next((c for c in map(_curve, CIRCOM_CURVES) if c.r == prime), None)
     if cv is None:
         raise ValueError("unknown field modulus")
     co, csize = sections[2]
@@ -122,7 +133,7 @@ def read_r1cs(data: bytes) -> R1CS:
 
 def write_witness(witness: Witness, public_inputs: List[Variable]) -> bytes:
     """witness.rs:27-104: one, outputs in index order, public inputs (BTreeSet order), then the rest in map order."""
-    c = witness.curve
+    c = _circom_curve(witness.curve)
     n8 = (c.r.bit_length() + 7) // 8
     w = dict(witness.values)
     vals = []
@@ -161,7 +172,7 @@ def read_wtns(data: bytes) -> Tuple[str, np.ndarray]:
     (n8,) = struct.unpack_from("<I", data, ho)
     prime = int.from_bytes(data[ho + 4:ho + 4 + n8], "little")
     (n,) = struct.unpack_from("<I", data, ho + 4 + n8)
-    cv = next((c for c in map(_curve, ("bn128", "bls12_381")) if c.r == prime), None)
+    cv = next((c for c in map(_curve, CIRCOM_CURVES) if c.r == prime), None)
     if cv is None:
         raise ValueError("unknown field modulus")
     do, dsize = sections[2]

@@ -9,6 +9,7 @@
 #if defined(ZKB_EMU)  // the host-emulation test build is a single translation unit
 #include "engine_bn254.cu"
 #include "engine_bls12_381.cu"
+#include "engine_bls12_377.cu"
 #endif
 
 using namespace zkb;
@@ -79,7 +80,8 @@ int32_t zkb_ctx_create(int32_t curve, int32_t device, zkb_ctx** out) {
   if (!out) { g_err = "out is null"; return ZKB_E_ARG; }
   *out = nullptr;
   try {
-    if (curve != ZKB_CURVE_BN128 && curve != ZKB_CURVE_BLS12_381) throw Error(ZKB_E_ARG, "unknown curve id");
+    if (curve != ZKB_CURVE_BN128 && curve != ZKB_CURVE_BLS12_381 && curve != ZKB_CURVE_BLS12_377)
+      throw Error(ZKB_E_ARG, "unknown curve id");
     std::unique_ptr<zkb_ctx> c(new zkb_ctx());
     c->curve = curve;
     c->device = device;
@@ -95,7 +97,9 @@ int32_t zkb_ctx_create(int32_t curve, int32_t device, zkb_ctx** out) {
     ZKB_CUDA(cudaSetDevice(device));
     ZKB_CUDA(cudaStreamCreateWithFlags(&c->st.s, cudaStreamNonBlocking));
 #endif
-    c->eng.reset(curve == ZKB_CURVE_BN128 ? make_engine_bn254(c->st) : make_engine_bls12_381(c->st));
+    c->eng.reset(curve == ZKB_CURVE_BN128       ? make_engine_bn254(c->st)
+                 : curve == ZKB_CURVE_BLS12_381 ? make_engine_bls12_381(c->st)
+                                                : make_engine_bls12_377(c->st));
     c->launches0 = launch_counter();
     *out = c.release();
     return ZKB_OK;
@@ -127,6 +131,8 @@ int32_t zkb_curve_sizes(int32_t curve, uint64_t out[4]) {
     out[0] = 32; out[1] = 32; out[2] = 256; out[3] = partial_bytes_bn254();
   } else if (curve == ZKB_CURVE_BLS12_381) {
     out[0] = 32; out[1] = 48; out[2] = 384; out[3] = partial_bytes_bls12_381();
+  } else if (curve == ZKB_CURVE_BLS12_377) {
+    out[0] = 32; out[1] = 48; out[2] = 384; out[3] = partial_bytes_bls12_377();
   } else {
     g_err = "unknown curve id";
     return ZKB_E_ARG;

@@ -1481,7 +1481,8 @@ class Engine : public EngineBase {
       // With three or more ranks the witness-map chains are computed once each by ranks 0, 1, 2 at the head of their main
       // stream (DESIGN.md §6): those ranks get a smaller share of the MSM work so that all ranks reach the h-MSM together.
       // f = one chain's cost as a fraction of the whole MSM work, from a cost model fitted at 2^20 (a chain = 0.19 n
-      // log2(n)/20 weight units in BN254, 0.086 in BLS12-381, a weight unit = one G1 point through all windows);
+      // log2(n)/20 weight units in BN254, 0.086 in BLS12-381, a weight unit = one G1 point through all windows; BLS12-377 has
+      // BLS12-381's limb counts and takes its figure, not re-fitted);
       // ZKB_OPT_CHAIN_SHARE: -1 model (default), 0 equal shares, > 0 f in 1/1000.
       std::vector<double> cum(world + 1, 0.0);
       {

@@ -81,10 +81,12 @@ struct EngineBase {
 };
 
 
-// one translation unit per curve (engine_bn254.cu / engine_bls12_381.cu)
+// one translation unit per curve (engine_bn254.cu / engine_bls12_381.cu / engine_bls12_377.cu)
 EngineBase* make_engine_bn254(Stream st);
 EngineBase* make_engine_bls12_381(Stream st);
+EngineBase* make_engine_bls12_377(Stream st);
 size_t partial_bytes_bn254();
 size_t partial_bytes_bls12_381();
+size_t partial_bytes_bls12_377();
 
 }  // namespace zkb

@@ -1,5 +1,5 @@
-// Montgomery-form prime-field arithmetic on 32-bit limbs (8 limbs: BN254 Fr/Fq, BLS12-381 Fr;
-// 12 limbs: BLS12-381 Fq).
+// Montgomery-form prime-field arithmetic on 32-bit limbs (8 limbs: BN254 Fr/Fq, BLS12-381 Fr, BLS12-377 Fr;
+// 12 limbs: BLS12-381 Fq, BLS12-377 Fq).
 //
 // Replaces, on the device, what the reference reaches through `zokrates_field::FieldPrime`
 // (/root/reference/zokrates_field/src/lib.rs:407-503 -> ark_ff::Fp256/Fp384 Montgomery ops, ark-ff
@@ -27,9 +27,20 @@
 
 namespace zkb {
 
+// beta of Fq2 = Fq[u]/(u^2 - beta): P::FP2_NONRESIDUE where the parameters define it (BLS12-377 Fq: -5), else -1
+template <class P, class = void>
+struct Fp2NonResidue {
+  static constexpr int value = -1;
+};
+template <class P>
+struct Fp2NonResidue<P, decltype((void)P::FP2_NONRESIDUE)> {
+  static constexpr int value = P::FP2_NONRESIDUE;
+};
+
 template <class P>
 struct alignas(16) Fp {
   static constexpr int N = P::N;
+  static constexpr int FP2_NONRESIDUE = Fp2NonResidue<P>::value;
   typedef P Params;
   uint32_t v[N];
 
@@ -191,6 +202,13 @@ struct alignas(16) Fp {
   // (redc's bound); products of unreduced sums < 2p, (2p)^2 = 4p^2 < p*R; and mul() with one operand < 2p, whose
   // running value < a + p < 3p must fit in N limbs (3p < R) and whose product < 2p^2 < p*R.
   static constexpr bool LAZY_HEADROOM = (P::mod(N - 1) >> 30) == 0;
+  // K p < R, evaluated on the modulus limbs (BN254 Fq: K <= 5, BLS12-381 Fq: K <= 9, BLS12-377 Fq: K <= 152)
+  template <int K>
+  ZKB_HD static constexpr bool fits_kp() {
+    uint64_t c = 0;
+    for (int i = 0; i < N; i++) c = ((uint64_t)P::mod(i) * K + c) >> 32;
+    return c == 0;
+  }
   struct Wide {
     uint32_t v[2 * N];
   };
@@ -356,9 +374,11 @@ struct alignas(16) Fp {
     r.v[2 * N - 1] = ptx::subc(a.v[2 * N - 1], b.v[2 * N - 1]);
     return r;
   }
+  // a + M p^2.  Callers add it to a sum of at most two products of reduced values (< 2p^2) before subtracting
+  // at most M p^2, so the operand of the following redc is < (M + 2) p^2, and (M + 2) p < R keeps it < p*R.
   template <int M>
-  ZKB_HD static Wide add_psq(const Wide& a) {  // a + M p^2; caller guarantees no overflow
-    static_assert(LAZY_HEADROOM && M <= 2, "M p^2 plus the operand must stay < p*R");
+  ZKB_HD static Wide add_psq(const Wide& a) {
+    static_assert(fits_kp<M + 2>(), "M p^2 plus the operand must stay < p*R");
     constexpr PSq<M> K{};
     Wide r;
     r.v[0] = ptx::add_cc(a.v[0], K.v[0]);
@@ -366,6 +386,14 @@ struct alignas(16) Fp {
     for (int i = 1; i < 2 * N - 1; i++) r.v[i] = ptx::addc_cc(a.v[i], K.v[i]);
     r.v[2 * N - 1] = ptx::addc(a.v[2 * N - 1], K.v[2 * N - 1]);
     return r;
+  }
+  // 5a as (a << 2) + a, for fp2.cuh's beta = -5 products; caller guarantees 5a < 2^(64N)
+  ZKB_HD static Wide mul5_wide(const Wide& a) {
+    Wide s;
+#pragma unroll
+    for (int k = 2 * N - 1; k >= 1; k--) s.v[k] = (a.v[k] << 2) | (a.v[k - 1] >> 30);
+    s.v[0] = a.v[0] << 2;
+    return add_wide(s, a);
   }
   // a + b without the conditional subtraction: < 2p for reduced inputs; only for mul_wide/mul operands
   ZKB_HD static Fp add_nr(const Fp& a, const Fp& b) {

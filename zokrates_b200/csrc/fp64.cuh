@@ -15,6 +15,7 @@ namespace zkb {
 template <class P>
 struct alignas(16) Fp64 {
   static constexpr int N = P::N / 2;
+  static constexpr int FP2_NONRESIDUE = Fp2NonResidue<P>::value;
   typedef P Params;
   typedef unsigned __int128 u128;
   uint64_t v[N];

@@ -177,7 +177,8 @@ struct ProgData {
 
 namespace prog_detail {
 
-static const uint8_t CURVE_ID[2][4] = {{0xb4, 0xf7, 0xb5, 0xbd}, {0x40, 0xd8, 0xc1, 0xf9}};   // zokrates_field/src/lib.rs:283-293
+static const uint8_t CURVE_ID[3][4] = {{0xb4, 0xf7, 0xb5, 0xbd}, {0x40, 0xd8, 0xc1, 0xf9},   // zokrates_field/src/lib.rs:283-293
+                                      {0xc2, 0x95, 0x5a, 0xb5}};                              // bn128, bls12_381, bls12_377
 
 inline uint32_t le32(const uint8_t* p) { return (uint32_t)p[0] | (uint32_t)p[1] << 8 | (uint32_t)p[2] << 16 | (uint32_t)p[3] << 24; }
 inline uint64_t le64(const uint8_t* p) { return (uint64_t)le32(p) | (uint64_t)le32(p + 4) << 32; }

@@ -37,6 +37,7 @@ ZKB_HD Affine<Fq2> std_g2() {
 template <class C> struct GenOf;
 template <> struct GenOf<CurveT<Bn254Fr, Bn254Fq>> { typedef Bn254Gen T; };
 template <> struct GenOf<CurveT<Bls381Fr, Bls381Fq>> { typedef Bls381Gen T; };
+template <> struct GenOf<CurveT<Bls377Fr, Bls377Fq>> { typedef Bls377Gen T; };
 
 // write one affine point in ark's uncompressed encoding (canonical LE, infinity flag 0x40 on the last byte)
 template <class F>

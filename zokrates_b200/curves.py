@@ -1,5 +1,5 @@
 """Curve / field constants the host side needs (names as `zokrates_field::Field::name()`,
-/root/reference/zokrates_field/src/bn128.rs:1-13, bls12_381.rs:1-13; moduli SURVEY.md App. C)."""
+/root/reference/zokrates_field/src/bn128.rs:1-13, bls12_381.rs:1-13, bls12_377.rs:1-13; moduli SURVEY.md App. C)."""
 from __future__ import annotations
 
 import hashlib
@@ -30,7 +30,10 @@ BN128 = Curve("bn128", 0, 218882428718392752222464057452572750885483644004160343
 BLS12_381 = Curve("bls12_381", 1, 0x73eda753299d7d483339d80809a1d80553bda402fffe5bfeffffffff00000001,
                   0x1a0111ea397fe69a4b1ba7b6434bacd764774b84f38512bf6730d2a0f6b0f6241eabfffeb153ffffb9feffffffffaaab,
                   32, 48, 1, 32, 7)
-CURVES = {"bn128": BN128, "bls12_381": BLS12_381}
+BLS12_377 = Curve("bls12_377", 2, 0x12ab655e9a2ca55660b44d1e5c37b00159aa76fed00000010a11800000000001,
+                  0x01ae3a4617c510eac63b05c06ca1493b1a22d9f300f5138f1ef3622fba094800170b5d44300000008508c00000000001,
+                  32, 48, 3, 47, 22)
+CURVES = {"bn128": BN128, "bls12_381": BLS12_381, "bls12_377": BLS12_377}
 
 
 def curve(name_or_curve) -> Curve:

@@ -132,11 +132,12 @@ def msm_g1_sharded(ctx, points: bytes, scalars: np.ndarray, group=None, device=N
     all-gathered (one point per rank) and added on the host.  Returns the point in ark's uncompressed encoding on every rank."""
     import torch
     import torch.distributed as dist
+    from .curves import CURVES
     from .verify import _pairing
     world, rank = dist.get_world_size(group), dist.get_rank(group)
     scalars = np.ascontiguousarray(scalars, dtype=np.uint64)
     n = scalars.shape[0]
-    curve_name = "bn128" if ctx.curve == 0 else "bls12_381"
+    curve_name = next(c.name for c in CURVES.values() if c.id == ctx.curve)
     pr = _pairing(curve_name)
     nb = 2 * pr.c.fq_bytes
     lo, hi = n * rank // world, n * (rank + 1) // world

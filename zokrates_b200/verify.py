@@ -3,10 +3,11 @@
 The reference verifies on the CPU (`zokrates_ark/src/groth16.rs:55-86`: rebuild the ark `VerifyingKey` from the hex
 fields, `prepare_verifying_key`, `verify_proof`, i.e. e(A, B) = e(alpha, beta) · e(Σ x_i·γ_abc_i, gamma) · e(C, delta)); it is
 milliseconds of work and SURVEY.md §8 row a13 keeps it off the GPU.  In the Rust shim `B200::verify` simply delegates to `Ark`.
-This module is the Python mirror's equivalent: a small, tower-free pairing over big integers (BN254 and BLS12-381), written for
-clarity, not speed (a verification takes a few seconds) — Fq12 is Fq[w] / (w^12 − 2a·w^6 + a² + 1) with the Fq2 unit
-i = w^6 − a (ξ = a + i the sextic non-residue: a = 9 for BN254, 1 for BLS12-381), G2 points are mapped through the twist
-into E(Fq12), and the Miller loop uses plain affine line functions.  Independent of `oracle/` (which the product never imports).
+This module is the Python mirror's equivalent: a small, tower-free pairing over big integers (BN254, BLS12-381 and BLS12-377),
+written for clarity, not speed (a verification takes a few seconds) — Fq12 is Fq[w] / (w^12 − 2a·w^6 + a² − β) with the Fq2
+unit u = w^6 − a, u² = β (ξ = a + u the sextic non-residue: β = −1 and a = 9 for BN254, β = −1 and a = 1 for BLS12-381,
+β = −5 and a = 0 for BLS12-377), G2 points are mapped through the twist into E(Fq12), and the Miller loop uses plain affine
+line functions.  Independent of `oracle/` (which the product never imports).
 """
 from __future__ import annotations
 
@@ -15,17 +16,18 @@ from typing import List, Optional, Tuple
 from .curves import curve as _curve
 from .proof import G1Affine, G2Affine, Proof, VerificationKey
 
-_PARAMS = {   # p, b of G1, a (xi = a + i), twist type, |ate loop count|, extra Frobenius lines (BN only)
-    "bn128": dict(b=3, a=9, mtwist=False, loop=29793968203157093288, bn=True),
-    "bls12_381": dict(b=4, a=1, mtwist=True, loop=15132376222941642752, bn=False),
+_PARAMS = {   # b of G1, beta (u^2), a (xi = a + u), twist type, |ate loop count|, extra Frobenius lines (BN only)
+    "bn128": dict(b=3, beta=-1, a=9, mtwist=False, loop=29793968203157093288, bn=True),
+    "bls12_381": dict(b=4, beta=-1, a=1, mtwist=True, loop=15132376222941642752, bn=False),
+    "bls12_377": dict(b=1, beta=-5, a=0, mtwist=False, loop=0x8508c00000000001, bn=False),
 }
 
 
 class _Fq12:
     """Arithmetic in Fq[w] / (w^12 + c6 w^6 + c0); elements are 12-tuples of ints."""
 
-    def __init__(self, p: int, a: int):
-        self.p, self.c6, self.c0 = p, (-2 * a) % p, (a * a + 1) % p
+    def __init__(self, p: int, a: int, beta: int = -1):
+        self.p, self.c6, self.c0 = p, (-2 * a) % p, (a * a - beta) % p
         self.one = (1,) + (0,) * 11
         self.zero = (0,) * 12
 
@@ -117,7 +119,7 @@ class _Pairing:
         self.c = _curve(name)
         self.P = _PARAMS[name]
         self.p = self.c.p
-        self.F = _Fq12(self.p, self.P["a"])
+        self.F = _Fq12(self.p, self.P["a"], self.P["beta"])
         w = [0] * 12
         w[1] = 1
         self.w = tuple(w)

@@ -28,7 +28,7 @@ from .ir import Constraint, Directive, LinComb, Log, Parameter, Prog, QuadComb, 
 
 MAGIC = b"ZOK\x00"
 VERSION = bytes([3, 0, 0, 0])
-CURVE_IDS = {"bn128": bytes.fromhex("b4f7b5bd"), "bls12_381": bytes.fromhex("40d8c1f9")}
+CURVE_IDS = {"bn128": bytes.fromhex("b4f7b5bd"), "bls12_381": bytes.fromhex("40d8c1f9"), "bls12_377": bytes.fromhex("c2955ab5")}
 HEADER_RESERVED = 120          # size_of::<ProgHeader>() on a 64-bit target: 20 + 4 * 24, rounded up to 8
 SECTION_TYPES = (1, 2, 3, 3)   # the module map is (mis)labelled Solvers by the reference writer
 
