@@ -100,6 +100,9 @@ int32_t zkb_pk_table_info(zkb_ctx* ctx, uint64_t pk_handle, uint64_t out[8]);
                                  * query vector at zkb_pk_load; -1 (default) from a cost model, 0 equal shares, > 0 the chain's cost in
                                  * 1/1000 of the whole MSM work.  Must be equal on all ranks (the cuts are derived independently). */
 #define ZKB_OPT_NTT_KERNEL 9    /* tile pass of the NTT: 2 (default) four-step twiddles + cp.async tile load, 1 the round-1 pass */
+#define ZKB_OPT_BATCH_PASS_MAX 15 /* most proofs zkb_groth16_prove_batch runs as one pass (one set of launches); 0 (default) = as many as
+                                   * fit in free HBM and in the 32-bit indices of the sorted MSM lists.  Larger batches run as several
+                                   * passes with the same proofs; tests use it to force several passes */
 #define ZKB_OPT_PK_CACHE 8      /* 1 (default): zkb_pk_load of bytes that are already resident returns a handle onto the same key
                                  * (content fingerprint), and the last key released by zkb_pk_free stays resident until another
                                  * key is loaded — the per-call pk_load / prove / pk_free of the static trait method then builds
@@ -133,6 +136,19 @@ int32_t zkb_groth16_prove(zkb_ctx* ctx, uint64_t pk_handle, uint64_t r1cs_handle
 int32_t zkb_r1cs_set_assignment(zkb_ctx* ctx, uint64_t r1cs_handle, const uint64_t* z);
 int32_t zkb_groth16_prove_resident(zkb_ctx* ctx, uint64_t pk_handle, uint64_t r1cs_handle,
                                    const uint64_t* r, const uint64_t* s, uint8_t* proof_out, size_t proof_cap);
+
+/* K proofs of one circuit under one key.  z: K full assignments back to back (K x (n_instance + n_witness) elements,
+ * canonical LE); r, s: K scalars each, canonical LE; proofs_out: K x zkb_curve_sizes()[2] bytes, proof k byte-identical
+ * to zkb_groth16_prove(pk, r1cs, z_k, r_k, s_k).
+ * The proofs share the key, its window tables, the matrices and the domain, so the device work of a PASS of proofs is one
+ * set of launches: one SpMV over all assignments, the transforms of all chain vectors at once, and MSMs with one bucket set
+ * per proof over the shared points.  A pass holds as many proofs as fit in free HBM (see ZKB_OPT_BATCH_PASS_MAX); the host
+ * tails of its proofs run in parallel on host threads.  From a domain of 2^18 on, where a batch gains nothing over the pipeline, and
+ * for count 1 the proofs run one after the other through the two-slot pipeline (zkb_groth16_prove_submit / _collect): same bytes.
+ * ZKB_E_ARG: count 0, proofs_out too small, a key loaded with world > 1, a proof in flight on this context (it stays
+ * collectable), a key that does not match the R1CS.  ZKB_E_OOM when not even one proof fits. */
+int32_t zkb_groth16_prove_batch(zkb_ctx* ctx, uint64_t pk_handle, uint64_t r1cs_handle, uint32_t count,
+                                const uint64_t* z, const uint64_t* r, const uint64_t* s, uint8_t* proofs_out, size_t cap);
 
 /* Multi-GPU: every rank computes the partial sums of its index slice (opaque blob, host memory,
  * zkb_curve_sizes()[3] bytes: five projective points — their representation depends on the order the sort's
@@ -219,7 +235,9 @@ int32_t zkb_witness_eval(zkb_ctx* ctx, uint64_t r1cs_handle, uint64_t* z_inout, 
  *   zkb_groth16_prove_resident.  ZKB_E_UNSAT + *first_unsatisfied on a violated constraint; ZKB_E_ARG "WrongInputCount".
  * zkb_prog_set_witness: `Witness::read` (:55-71) of a witness file into the resident assignment (ark column order).
  * zkb_prog_public_inputs: public arguments in declaration order, then ~out_0.. (ir/mod.rs:278-288) of the current
- *   assignment, canonical, 32 bytes each; out may be NULL to query *count. */
+ *   assignment, canonical, 32 bytes each; out may be NULL to query *count.
+ * zkb_prog_assignment: the program's current assignment (after zkb_prog_set_witness / zkb_prog_compute_witness) in ark
+ *   column order, host copy: n_instance + n_witness canonical LE elements (4 x u64 each); cap_elems counts elements. */
 int32_t zkb_prog_load(zkb_ctx* ctx, const uint8_t* out_bytes, size_t len, uint64_t* prog_handle);
 int32_t zkb_prog_info(zkb_ctx* ctx, uint64_t prog_handle, uint64_t out[12]);
 int32_t zkb_prog_free(zkb_ctx* ctx, uint64_t prog_handle);
@@ -227,6 +245,7 @@ int32_t zkb_prog_compute_witness(zkb_ctx* ctx, uint64_t prog_handle, const uint6
                                  uint8_t* witness_out, size_t witness_cap, size_t* witness_len, uint64_t* first_unsatisfied);
 int32_t zkb_prog_set_witness(zkb_ctx* ctx, uint64_t prog_handle, const uint8_t* witness_bytes, size_t len);
 int32_t zkb_prog_public_inputs(zkb_ctx* ctx, uint64_t prog_handle, uint64_t* out, uint64_t cap, uint64_t* count);
+int32_t zkb_prog_assignment(zkb_ctx* ctx, uint64_t prog_handle, uint64_t* z_out, uint64_t cap_elems);
 
 /* ---- GM17 (SURVEY.md §8 row f3) ------------------------------------------------------------------------
  * The second proving scheme of the same trait: `impl Backend<T, GM17> for Ark` (zokrates_ark/src/gm17.rs:43-75 ->

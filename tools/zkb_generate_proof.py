@@ -5,6 +5,7 @@ zokrates_cli/src/cli_constants.rs): reads the compiled program (`out`), the bina
 proves on the GPU (libzkb200.so — no CPU path) and writes `proof.json` in the reference's TaggedProof layout.
 
     python tools/zkb_generate_proof.py -i out -w witness -p proving.key -j proof.json [-e entropy] [--verbose]
+    python tools/zkb_generate_proof.py -i out --witnesses w0 w1 .. -p proving.key --proof-dir DIR [-e entropy]
 """
 import argparse
 import os
@@ -25,8 +26,14 @@ def main(argv=None) -> int:
     ap.add_argument("--device", type=int, default=0)
     ap.add_argument("--tables", type=int, default=0, choices=[0, 1],
                     help="build the HBM window tables for this key (pays off from about a hundred proofs per key on; a one-shot process proves without)")
+    ap.add_argument("--witnesses", nargs="+", default=None, metavar="FILE",
+                    help="prove several witness files of the program in one GPU batch (with --proof-dir; replaces -w / -j)")
+    ap.add_argument("--proof-dir", default=None, metavar="DIR",
+                    help="with --witnesses: write DIR/proof_<i>.json for the i-th witness (i from 0, in the order given)")
     ap.add_argument("--verbose", action="store_true")
     args = ap.parse_args(argv)
+    if (args.witnesses is None) != (args.proof_dir is None):
+        ap.error("--witnesses and --proof-dir go together")
 
     from zokrates_b200 import backend, rng, zir
     from zokrates_b200._lib import ZkbError
@@ -43,6 +50,26 @@ def main(argv=None) -> int:
         curve_name = zir.read_header(out_bytes)[0]          # only the header is read here; the library parses the rest
     except zir.ZirFormatError as why:
         raise SystemExit(str(why))
+    if args.witnesses is not None:
+        print(f"Generating {len(args.witnesses)} proofs...")
+        witnesses = [slurp(p) for p in args.witnesses]
+        pk = slurp(args.proving_key_path)
+        r = rng.get_rng_from_entropy(args.entropy) if args.entropy is not None else rng.StdRng.from_entropy()
+        try:
+            from zokrates_b200._lib import OPT_TABLES
+            backend.context(curve_name, args.device).set_option(OPT_TABLES, args.tables)
+            proofs = backend.B200.generate_proofs_files(out_bytes, witnesses, pk, r, curve=curve_name, device=args.device)
+        except ZkbError as why:
+            raise SystemExit(f"Could not generate the proofs: {why}")
+        try:
+            os.makedirs(args.proof_dir, exist_ok=True)
+            for i, proof in enumerate(proofs):
+                with open(os.path.join(args.proof_dir, f"proof_{i}.json"), "w") as f:
+                    f.write(proof.to_tagged_json())
+        except OSError as why:
+            raise SystemExit(f"Could not write to {args.proof_dir}: {why.strerror}")
+        print(f"{len(proofs)} proofs written to '{args.proof_dir}'")
+        return 0
     print("Generating proof...")
     witness_bytes = slurp(args.witness)
     pk = slurp(args.proving_key_path)

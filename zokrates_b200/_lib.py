@@ -31,9 +31,11 @@ SYMBOLS = [
     "zkb_groth16_prove_chains_to_stream", "zkb_groth16_prove_stream_to_finish",
     "zkb_prog_load", "zkb_prog_info", "zkb_prog_free", "zkb_prog_compute_witness", "zkb_prog_set_witness",
     "zkb_prog_public_inputs", "zkb_gm17_pk_load", "zkb_gm17_pk_free", "zkb_gm17_prove", "zkb_gm17_setup", "zkb_gm17_setup_size",
+    "zkb_groth16_prove_batch", "zkb_prog_assignment",
 ]
 
 OPT_TABLES, OPT_TABLE_MIN_LOG, OPT_TABLE_C, OPT_Z_MODE, OPT_NTT_TILE_MIN, OPT_NTT_MAX_S, OPT_BITSUM_RADIX, OPT_PK_CACHE, OPT_NTT_KERNEL, OPT_BATCH_AFFINE, OPT_BATCH_AFFINE_MIN_LOG = 1, 2, 3, 4, 5, 6, 7, 8, 9, 10, 11
+OPT_BATCH_PASS_MAX = 15
 TABLE_STATUS = {0: "none", 1: "built", 2: "below-min-size", 3: "no-memory", 4: "disabled", 5: "no-window"}
 
 
@@ -78,6 +80,9 @@ class Library:
         d.zkb_r1cs_set_assignment.argtypes = [C.c_void_p, C.c_uint64, C.c_void_p]
         d.zkb_groth16_prove.argtypes = [C.c_void_p, C.c_uint64, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p,
                                         C.c_void_p, C.c_size_t]
+        d.zkb_groth16_prove_batch.argtypes = [C.c_void_p, C.c_uint64, C.c_uint64, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p,
+                                              C.c_void_p, C.c_size_t]
+        d.zkb_prog_assignment.argtypes = [C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64]
         d.zkb_groth16_prove_resident.argtypes = [C.c_void_p, C.c_uint64, C.c_uint64, C.c_void_p, C.c_void_p,
                                                  C.c_void_p, C.c_size_t]
         d.zkb_groth16_prove_partial.argtypes = [C.c_void_p, C.c_uint64, C.c_uint64, C.c_void_p, C.c_void_p, C.c_size_t]
@@ -242,6 +247,23 @@ class Context:
                                                       out.ctypes.data, len(out)))
         return out.tobytes()
 
+    def prove_batch(self, pk, r1cs, zs, rs, ss) -> list:
+        """K proofs of one circuit in one call (zkb_groth16_prove_batch): zs holds K assignments (a (K, m, 4) array or a list
+        of (m, 4) arrays), rs / ss K scalars each.  Proof k is byte-identical to prove(pk, r1cs, zs[k], rs[k], ss[k])."""
+        if isinstance(zs, np.ndarray) and zs.dtype == np.uint64 and zs.ndim == 3 and zs.flags.c_contiguous:
+            z = zs                    # already K assignments back to back: no copy
+        else:
+            z = np.ascontiguousarray(np.stack([np.asarray(x, dtype=np.uint64).reshape(-1, 4) for x in zs]) if len(zs) else
+                                     np.zeros((0, 4), dtype=np.uint64), dtype=np.uint64)
+        k = len(zs)
+        if len(rs) != k or len(ss) != k:
+            raise ValueError("zs, rs and ss must have the same length")
+        ra, sa = fr_array(list(rs)), fr_array(list(ss))
+        out = np.zeros(max(k, 1) * self.proof_bytes, dtype=np.uint8)
+        self.lib.check(self.lib.dll.zkb_groth16_prove_batch(self.h, pk, r1cs, k, z.ctypes.data, ra.ctypes.data, sa.ctypes.data,
+                                                            out.ctypes.data, k * self.proof_bytes))
+        return [out[i * self.proof_bytes:(i + 1) * self.proof_bytes].tobytes() for i in range(k)]
+
     def prove_resident(self, pk, r1cs, r: int, s: int) -> bytes:
         ra, sa = fr_array([r]), fr_array([s])
         out = np.zeros(self.proof_bytes, dtype=np.uint8)
@@ -401,6 +423,14 @@ class Context:
         out = np.zeros((max(n.value, 1), 4), dtype=np.uint64)
         self.lib.check(self.lib.dll.zkb_prog_public_inputs(self.h, prog, out.ctypes.data, n.value, C.byref(n)))
         return fr_from_array(out[:n.value])
+
+    def prog_assignment(self, prog: int) -> np.ndarray:
+        """The program's current assignment (after prog_set_witness / prog_compute_witness), ark column order, (m, 4) uint64."""
+        info = self.prog_info(prog)
+        m = info["instance"] + info["witness"]
+        out = np.zeros((m, 4), dtype=np.uint64)
+        self.lib.check(self.lib.dll.zkb_prog_assignment(self.h, prog, out.ctypes.data, m))
+        return out
 
     # -- GM17
     def gm17_setup(self, r1cs: int, trapdoor6) -> bytes:

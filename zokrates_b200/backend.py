@@ -143,6 +143,67 @@ class B200:
         return Proof.from_raw(c, raw, inputs)
 
     @staticmethod
+    def generate_proofs(program: Prog, witnesses, proving_key, rng: StdRng, device: int = 0,
+                        lib: Optional[_lib.Library] = None) -> list:
+        """Proofs of several witnesses of ONE program under one key, proved as one batch on the GPU (zkb_groth16_prove_batch).
+        (r, s) are drawn for the first witness, then the second, and so on, so with the same rng state the result equals
+        `[B200.generate_proof(program, w, proving_key, rng) for w in witnesses]`.  An addition beside the trait, which has
+        no batch method."""
+        c = _curve(program.curve)
+        pk_bytes = proving_key.read() if hasattr(proving_key, "read") else bytes(proving_key)
+        r1cs = synthesize(program)
+        inputs, zs, rs, ss = [], [], [], []
+        for w in witnesses:
+            inputs.append(program.public_inputs_values(w))
+            rs.append(fr_rand(c, rng))
+            ss.append(fr_rand(c, rng))
+            try:
+                zs.append(r1cs.assignment(w))
+            except KeyError as e:
+                raise RuntimeError(f"AssignmentMissing: {e}")
+        if not zs:
+            return []
+        sess = ProverSession(c, r1cs, pk_bytes, device, lib=lib)
+        try:
+            raws = sess.ctx.prove_batch(sess.pk_h, sess.r1cs_h, zs, rs, ss)
+        finally:
+            sess.close()
+        return [Proof.from_raw(c, raw, inp) for raw, inp in zip(raws, inputs)]
+
+    @staticmethod
+    def generate_proofs_files(out_bytes: bytes, witness_bytes_list, proving_key, rng: StdRng, curve="bn128", device: int = 0,
+                              lib: Optional[_lib.Library] = None) -> list:
+        """`generate_proof_files` for several witness FILES of one program: every witness is read natively
+        (`zkb_prog_set_witness`, `zkb_prog_assignment`, `zkb_prog_public_inputs`) and all of them are proved in one batch.
+        (r, s) are drawn in witness order, so the proofs equal sequential `generate_proof_files` calls on the same rng."""
+        c = _curve(curve)
+        ctx = context(c, device, lib)
+        pk_bytes = proving_key.read() if hasattr(proving_key, "read") else proving_key
+        rs, ss = [], []
+        for _ in witness_bytes_list:
+            rs.append(fr_rand(c, rng))
+            ss.append(fr_rand(c, rng))
+        if not rs:
+            return []
+        with ctx.lock:
+            prog = ctx.prog_load(out_bytes)
+            pk_h = None
+            try:
+                info = ctx.prog_info(prog)
+                zs, inputs = [], []
+                for wb in witness_bytes_list:
+                    ctx.prog_set_witness(prog, wb)
+                    zs.append(ctx.prog_assignment(prog))
+                    inputs.append(ctx.prog_public_inputs(prog))
+                pk_h = ctx.pk_load(pk_bytes, 0, 1)
+                raws = ctx.prove_batch(pk_h, info["r1cs"], zs, rs, ss)
+            finally:
+                if pk_h:
+                    ctx.pk_free(pk_h)
+                ctx.prog_free(prog)
+        return [Proof.from_raw(c, raw, inp) for raw, inp in zip(raws, inputs)]
+
+    @staticmethod
     def setup_gm17(program: Prog, trapdoor, device: int = 0, lib: Optional[_lib.Library] = None) -> bytes:
         """`impl NonUniversalBackend<T, GM17> for Ark`::setup (zokrates_ark/src/gm17.rs:19-41) on the GPU.  `trapdoor`: an `StdRng`
         (alpha, beta, gamma, tau and the two generator scalars are drawn with `fr_rand`, in that order) or 6 explicit integers.

@@ -170,6 +170,7 @@ int32_t zkb_ctx_set_option(zkb_ctx* ctx, int32_t opt, int64_t value) {
       case ZKB_OPT_NTT_KERNEL: if (value != 1 && value != 2) throw Error(ZKB_E_ARG, "ZKB_OPT_NTT_KERNEL: 1 or 2"); o.ntt_kernel = value; break;
       case ZKB_OPT_PK_CACHE: if (value < 0 || value > 1) throw Error(ZKB_E_ARG, "ZKB_OPT_PK_CACHE: 0 or 1"); o.pk_cache = value; break;
       case ZKB_OPT_BITSUM_RADIX: if (value != 2 && value != 8) throw Error(ZKB_E_ARG, "ZKB_OPT_BITSUM_RADIX: 2 or 8"); o.bitsum_radix = value; break;
+      case ZKB_OPT_BATCH_PASS_MAX: if (value < 0 || value > 0xFFFFFFFFll) throw Error(ZKB_E_ARG, "ZKB_OPT_BATCH_PASS_MAX: 0 or a proof count"); o.batch_pass_max = value; break;
       default: throw Error(ZKB_E_ARG, "unknown option");
     }
   });
@@ -211,6 +212,17 @@ int32_t zkb_groth16_prove(zkb_ctx* ctx, uint64_t pk, uint64_t r1cs, const uint64
   return guard(ctx, [&] {
     if (!z) throw Error(ZKB_E_ARG, "null assignment");
     prove_common(ctx, pk, r1cs, z, r, s, proof_out, cap);
+  });
+}
+int32_t zkb_groth16_prove_batch(zkb_ctx* ctx, uint64_t pk, uint64_t r1cs, uint32_t count, const uint64_t* z, const uint64_t* r,
+                                const uint64_t* s, uint8_t* proofs_out, size_t cap) {
+  return guard(ctx, [&] {
+    if (count == 0) throw Error(ZKB_E_ARG, "empty batch");
+    if (!z || !r || !s || !proofs_out) throw Error(ZKB_E_ARG, "null argument");
+    uint64_t sz[4];
+    ctx->eng->sizes(sz);
+    if (cap / count < sz[2]) throw Error(ZKB_E_ARG, "proofs_out too small");
+    ctx->eng->prove_batch(pk, r1cs, count, z, r, s, proofs_out);
   });
 }
 int32_t zkb_groth16_prove_resident(zkb_ctx* ctx, uint64_t pk, uint64_t r1cs, const uint64_t* r, const uint64_t* s,
@@ -358,6 +370,12 @@ int32_t zkb_prog_public_inputs(zkb_ctx* ctx, uint64_t h, uint64_t* out, uint64_t
   return guard(ctx, [&] {
     uint64_t n = ctx->eng->prog_public_inputs(h, out, cap);
     if (count) *count = n;
+  });
+}
+int32_t zkb_prog_assignment(zkb_ctx* ctx, uint64_t h, uint64_t* z_out, uint64_t cap_elems) {
+  return guard(ctx, [&] {
+    if (!z_out) throw Error(ZKB_E_ARG, "null argument");
+    ctx->eng->prog_assignment(h, z_out, cap_elems);
   });
 }
 int32_t zkb_gm17_pk_load(zkb_ctx* ctx, const uint8_t* pk_bytes, size_t len, uint64_t* h) {

@@ -14,6 +14,7 @@
 #include <chrono>
 #include <cmath>
 #include <future>
+#include <thread>
 #include "fp64.cuh"
 #include "msm.cuh"
 #include "msm_affine.cuh"
@@ -248,7 +249,7 @@ static __global__ void __launch_bounds__(VIEW_BLOCK) zkb_view_apply(MsmShape sh,
 
 // ---------------------------------------------------------------------------------------------
 struct MsmPlan {
-  MsmShape sh{0, 0, 0, 0, 0};
+  MsmShape sh{0, 0, 0, 0, 0, 1};
   uint32_t nbuckets = 0;
   uint32_t T1 = 32, T2 = 32;
   uint32_t nt1 = 0;  // level-1 chunks
@@ -405,12 +406,14 @@ class Engine : public EngineBase {
     return sm_count_ ? sm_count_ : 1;
   }
 
-  // natural -> bit-reversed
-  void ntt_dif(Fr* x, const Fr* tw, uint32_t log_n) {
+  // natural -> bit-reversed.  `count` vectors of 2^log_n elements back to back (a batch of proofs): every launch transforms
+  // all of them with the same twiddles, a thread or tile finds its vector from its index.
+  void ntt_dif(Fr* x, const Fr* tw, uint32_t log_n, uint32_t count = 1) {
     NttPass ps[8];
     const uint32_t np = ntt_tiled(log_n) ? ntt_plan_passes(log_n, ntt_max_s(), ps) : 0;
     if (np) {
-      const size_t tiles = ((size_t)1 << log_n) >> NTT_TILE_LOG;
+      const uint32_t lg_tpv = log_n - NTT_TILE_LOG;
+      const size_t tiles = (size_t)count << lg_tpv;
       const Fr* nul = nullptr;
 #if !defined(ZKB_EMU)
       if (opts.ntt_kernel == 2) {           // four-step twiddles, cp.async tile load, padded planes (ntt_tile.cuh)
@@ -421,29 +424,32 @@ class Engine : public EngineBase {
       for (uint32_t i = 0; i < np; i++) {   // top stage bits first
         NttPass p = ps[i];
         launch_block<k_ntt_dif_tile, NTT_BLOCK, NTT_TILE * sizeof(Fr)>(st_, tiles, p.nk + 2, ZKB_LAMBDA(uint32_t b, uint32_t t, uint32_t ph, void* sm) {
-          ntt_block_body<Fr, false>(x, tw, nul, p, (Fr*)sm, b, t, ph);
+          ntt_block_body<Fr, false>(x + ((size_t)(b >> lg_tpv) << log_n), tw, nul, p, (Fr*)sm, b & ((1u << lg_tpv) - 1u), t, ph);
         });
       }
       return;
     }
     uint32_t h = (1u << log_n) >> 1, rem = log_n;
-    const size_t n = (size_t)1 << log_n;
+    const size_t cn = (size_t)count << log_n;
     while (rem > 0) {
       uint32_t K = rem >= 3 ? 3 : rem;
       uint32_t h0 = h;
-      if (K == 3) launch<k_ntt_dif>(st_, n >> 3, ZKB_LAMBDA(size_t t) { ntt_dif_body<Fr, 3>(x, tw, log_n, h0, (uint32_t)t); });
-      else if (K == 2) launch<k_ntt_dif>(st_, n >> 2, ZKB_LAMBDA(size_t t) { ntt_dif_body<Fr, 2>(x, tw, log_n, h0, (uint32_t)t); });
-      else launch<k_ntt_dif>(st_, n >> 1, ZKB_LAMBDA(size_t t) { ntt_dif_body<Fr, 1>(x, tw, log_n, h0, (uint32_t)t); });
+      // thread t of the launch: vector t >> (log_n - K), butterfly group t mod 2^(log_n - K)
+      const uint32_t lg = log_n - K;
+      if (K == 3) launch<k_ntt_dif>(st_, cn >> 3, ZKB_LAMBDA(size_t t) { ntt_dif_body<Fr, 3>(x + ((t >> lg) << log_n), tw, log_n, h0, (uint32_t)(t & ((1u << lg) - 1u))); });
+      else if (K == 2) launch<k_ntt_dif>(st_, cn >> 2, ZKB_LAMBDA(size_t t) { ntt_dif_body<Fr, 2>(x + ((t >> lg) << log_n), tw, log_n, h0, (uint32_t)(t & ((1u << lg) - 1u))); });
+      else launch<k_ntt_dif>(st_, cn >> 1, ZKB_LAMBDA(size_t t) { ntt_dif_body<Fr, 1>(x + ((t >> lg) << log_n), tw, log_n, h0, (uint32_t)(t & ((1u << lg) - 1u))); });
       h >>= K;
       rem -= K;
     }
   }
   // bit-reversed -> natural; `scale` (optional): x[i] *= scale[bitrev(i)] first (the coset shift between ifft and coset fft)
-  void ntt_dit(Fr* x, const Fr* tw, uint32_t log_n, const Fr* scale = nullptr) {
+  void ntt_dit(Fr* x, const Fr* tw, uint32_t log_n, const Fr* scale = nullptr, uint32_t count = 1) {
     NttPass ps[8];
     const uint32_t np = ntt_tiled(log_n) ? ntt_plan_passes(log_n, ntt_max_s(), ps) : 0;
     if (np) {
-      const size_t tiles = ((size_t)1 << log_n) >> NTT_TILE_LOG;
+      const uint32_t lg_tpv = log_n - NTT_TILE_LOG;
+      const size_t tiles = (size_t)count << lg_tpv;
 #if !defined(ZKB_EMU)
       if (opts.ntt_kernel == 2) {
         for (uint32_t i = np; i-- > 0;) launch_ntt_tile2<Fr, true>(st_, x, tw, (i == np - 1) ? scale : nullptr, ps[i], tiles, sm_count());
@@ -454,20 +460,22 @@ class Engine : public EngineBase {
         NttPass p = ps[i];
         const Fr* sc = (i == np - 1) ? scale : nullptr;
         launch_block<k_ntt_dit_tile, NTT_BLOCK, NTT_TILE * sizeof(Fr)>(st_, tiles, p.nk + 2, ZKB_LAMBDA(uint32_t b, uint32_t t, uint32_t ph, void* sm) {
-          ntt_block_body<Fr, true>(x, tw, sc, p, (Fr*)sm, b, t, ph);
+          ntt_block_body<Fr, true>(x + ((size_t)(b >> lg_tpv) << log_n), tw, sc, p, (Fr*)sm, b & ((1u << lg_tpv) - 1u), t, ph);
         });
       }
       return;
     }
-    if (scale) launch<k_ntt_scale>(st_, (size_t)1 << log_n, ZKB_LAMBDA(size_t t) { ntt_scale_brev_body<Fr>(x, scale, log_n, (uint32_t)t); });
+    const size_t cn = (size_t)count << log_n;
+    const uint32_t nmask = (1u << log_n) - 1u;
+    if (scale) launch<k_ntt_scale>(st_, cn, ZKB_LAMBDA(size_t t) { ntt_scale_brev_body<Fr>(x + ((t >> log_n) << log_n), scale, log_n, (uint32_t)(t & nmask)); });
     uint32_t h = 1, rem = log_n;
-    const size_t n = (size_t)1 << log_n;
     while (rem > 0) {
       uint32_t K = rem >= 3 ? 3 : rem;
       uint32_t h0 = h;
-      if (K == 3) launch<k_ntt_dit>(st_, n >> 3, ZKB_LAMBDA(size_t t) { ntt_dit_body<Fr, 3>(x, tw, log_n, h0, (uint32_t)t); });
-      else if (K == 2) launch<k_ntt_dit>(st_, n >> 2, ZKB_LAMBDA(size_t t) { ntt_dit_body<Fr, 2>(x, tw, log_n, h0, (uint32_t)t); });
-      else launch<k_ntt_dit>(st_, n >> 1, ZKB_LAMBDA(size_t t) { ntt_dit_body<Fr, 1>(x, tw, log_n, h0, (uint32_t)t); });
+      const uint32_t lg = log_n - K;
+      if (K == 3) launch<k_ntt_dit>(st_, cn >> 3, ZKB_LAMBDA(size_t t) { ntt_dit_body<Fr, 3>(x + ((t >> lg) << log_n), tw, log_n, h0, (uint32_t)(t & ((1u << lg) - 1u))); });
+      else if (K == 2) launch<k_ntt_dit>(st_, cn >> 2, ZKB_LAMBDA(size_t t) { ntt_dit_body<Fr, 2>(x + ((t >> lg) << log_n), tw, log_n, h0, (uint32_t)(t & ((1u << lg) - 1u))); });
+      else launch<k_ntt_dit>(st_, cn >> 1, ZKB_LAMBDA(size_t t) { ntt_dit_body<Fr, 1>(x + ((t >> lg) << log_n), tw, log_n, h0, (uint32_t)(t & ((1u << lg) - 1u))); });
       h <<= K;
       rem -= K;
     }
@@ -671,18 +679,21 @@ class Engine : public EngineBase {
     }
     tm.end();
   }
-  void wm_finish(R1cs& r, ProofSlot& sl, StageTimer& tm) {
+  // `count` proofs: vector k of a, b, c and h at offset k n (the chains of a batch are back to back)
+  void wm_finish(R1cs& r, Fr* pa, const Fr* pb, const Fr* pc, Fr* ph, uint32_t count, StageTimer& tm, const char* name) {
     DomainT& d = domain(r.log_n);
     const uint32_t lg = r.log_n;
-    const size_t n = (size_t)1 << lg;
-    tm.begin("witness_map_finish");
-    Fr* pa = sl.a.p; const Fr* pb = sl.b.p; const Fr* pc = sl.c.p;
+    const size_t cn = (size_t)count << lg;
+    tm.begin(name);
     Fr zinv = d.zinv;
-    launch<k_qap_pointwise>(st_, n, ZKB_LAMBDA(size_t t) { qap_pointwise_body<Fr>(pa, pb, pc, zinv, (uint32_t)n, (uint32_t)t); });
-    ntt_dif(pa, d.tw_inv.p, lg);
-    Fr* ph = sl.h.p;
+    launch<k_qap_pointwise>(st_, cn, ZKB_LAMBDA(size_t t) { qap_pointwise_body<Fr>(pa, pb, pc, zinv, (uint32_t)cn, (uint32_t)t); });
+    ntt_dif(pa, d.tw_inv.p, lg, count);
     const Fr* t2 = d.cos_inv.p;
-    launch<k_ntt_brev>(st_, n, ZKB_LAMBDA(size_t t) { ntt_brev_copy_body<Fr>(pa, ph, t2, lg, 1, (uint32_t)t); });
+    const uint32_t nmask = (1u << lg) - 1u;
+    launch<k_ntt_brev>(st_, cn, ZKB_LAMBDA(size_t t) {
+      const size_t base = (t >> lg) << lg;
+      ntt_brev_copy_body<Fr>(pa + base, ph + base, t2, lg, 1, (uint32_t)(t & nmask));
+    });
     tm.end();
   }
 
@@ -698,7 +709,7 @@ class Engine : public EngineBase {
     sl.z_src = sl.z_canon.p;
     tm.begin("witness_map");
     wm_chains(r, sl, 7, tm);
-    wm_finish(r, sl, tm);
+    wm_finish(r, sl.a.p, sl.b.p, sl.c.p, sl.h.p, 1, tm, "witness_map_finish");
     tm.end();
     d2h(st_, h_out, sl.h.p, n * FRB);
     stream_sync(st_);
@@ -937,6 +948,13 @@ class Engine : public EngineBase {
     witness_parse(p.d, wit, len, mod, p.z_host);
     set_assignment(p.d.r1cs, p.z_host.data());
   }
+  // the current assignment of the program (ark column order), as the last compute_witness / set_witness left it
+  void prog_assignment(uint64_t h, uint64_t* z_out, uint64_t cap_elems) override {
+    ProgDev& p = get_prog(h);
+    if (p.z_host.size() != (size_t)p.d.m * 4) throw Error(ZKB_E_ARG, "the program has no assignment yet");
+    if (cap_elems < p.d.m) throw Error(ZKB_E_ARG, "assignment buffer too small");
+    memcpy(z_out, p.z_host.data(), p.z_host.size() * 8);
+  }
   // public arguments in declaration order, then the return values ~out_0.. (ir/mod.rs:278-288), from the current assignment
   uint64_t prog_public_inputs(uint64_t h, uint64_t* out, uint64_t cap) override {
     ProgDev& p = get_prog(h);
@@ -960,19 +978,30 @@ class Engine : public EngineBase {
 
   // ------------------------------------------------------------------------------ MSM
 
+  // window width of an MSM of n pairs: the table's c, or the cost model's
+  static uint32_t plan_c(uint64_t n, uint32_t pre_c) { return pre_c ? pre_c : msm_pick_c(n, C::FR_BITS); }
+  static uint32_t plan_w(uint32_t c) { return (C::FR_BITS + 1 + c - 1) / c; }
+  // The sorted lists index (pair, window) entries of all proofs and views with uint32 offsets: the largest batch one plan holds
+  static uint64_t plan_max_batch(uint64_t n, uint32_t nviews, uint32_t pre_c) {
+    const uint64_t per = n * plan_w(plan_c(n, pre_c)) * nviews;
+    return per ? ((1ull << 32) - 1) / per : ~0ull;
+  }
+
+  // K > 1: a batch of K scalar vectors, vector k at scalars + k * stride (MsmShape)
   void plan_build(MsmPlan& pl, const Fr* scalars, uint64_t n, uint32_t nviews = 1, const uint8_t* skip = nullptr,
-                  uint32_t pre_c = 0 /* != 0: precomputed window tables with this c */) {
+                  uint32_t pre_c = 0 /* != 0: precomputed window tables with this c */, uint32_t K = 1, size_t stride = 0) {
     pl.sh.n = (uint32_t)n;
+    pl.sh.K = K;
     pl.nviews = nviews;
     pl.sh.pre = pre_c ? 1 : 0;
     if (n == 0) return;
-    uint32_t c = pre_c ? pre_c : msm_pick_c(n, C::FR_BITS);
+    uint32_t c = plan_c(n, pre_c);
     pl.sh.c = c;
-    pl.sh.W = (C::FR_BITS + 1 + c - 1) / c;
+    pl.sh.W = plan_w(c);
     pl.sh.B = 1u << (c - 1);
     pl.nbuckets = msm_nbuckets(pl.sh);
-    uint64_t total = n * pl.sh.W;
-    if (total * nviews >= (1ull << 32)) throw Error(ZKB_E_ARG, "msm too large");
+    uint64_t total = (uint64_t)K * n * pl.sh.W;
+    if (K == 0 || total * nviews >= (1ull << 32)) throw Error(ZKB_E_ARG, "msm too large");
     // chunk size: aim for several waves of resident threads, at least 8 entries per chunk
     uint64_t target = (uint64_t)opts.chunk_target;
     uint64_t T = (total + target - 1) / target;
@@ -991,11 +1020,11 @@ class Engine : public EngineBase {
     const uint32_t* sc = (const uint32_t*)scalars;
     uint32_t* dg = pl.digits.p; uint32_t* rk = pl.ranks.p; uint32_t* cn = pl.counts.p; uint32_t* of = pl.offsets.p;
     uint32_t* so = pl.sorted.p;
-    launch<k_msm_digits>(st_, n, ZKB_LAMBDA(size_t t) { msm_digits_body(sh, sc, dg, rk, cn, (uint32_t)t); });
+    launch<k_msm_digits>(st_, (size_t)K * n, ZKB_LAMBDA(size_t t) { msm_digits_body(sh, sc, stride, dg, rk, cn, (uint32_t)t); });
     const uint32_t ntiles = (uint32_t)((total + VIEW_TILE - 1) / VIEW_TILE);
     pl.scan_tmp.ensure(2 * ((size_t)(NB > ntiles ? NB : ntiles) / 2048 + 4));
     exclusive_scan(st_, cn, of, NB, pl.scan_tmp.p);
-    launch<k_msm_scatter>(st_, total, ZKB_LAMBDA(size_t t) { msm_scatter_body(sh, dg, rk, of, so, t); });
+    launch<k_msm_scatter>(st_, total, ZKB_LAMBDA(size_t t) { msm_scatter_body(sh, dg, rk, of, so, (uint32_t)t); });
     if (nviews > 1) build_views(pl, skip, total, ntiles);
   }
 
@@ -1056,6 +1085,7 @@ class Engine : public EngineBase {
     if (prepared_.fut.valid()) prepared_.fut.wait();
     for (auto& sl : slots_) { if (sl.fm.valid()) sl.fm.wait(); sl.destroy(); }
     ws_misc_.destroy();
+    batch_.destroy();
     if (has_wm_stream_) stream_destroy(wm_stream_);
     if (has_plan_stream_) stream_destroy(plan_stream_);
   }
@@ -1075,8 +1105,8 @@ class Engine : public EngineBase {
     ws.buckets.ensure((size_t)NB * sizeof(X));
     X* buckets = (X*)ws.buckets.p;
     const uint32_t* of = pl.offsets.p + (size_t)view * (NB + 1);
-    const uint32_t* so = pl.sorted.p + (size_t)view * pl.sh.n * pl.sh.W;
-    uint64_t bound = (uint64_t)pl.sh.n * pl.sh.W;          // upper bound of the list length (the exact length is offsets[NB], on the device)
+    uint64_t bound = (uint64_t)pl.sh.K * pl.sh.n * pl.sh.W;   // upper bound of the list length (the exact length is offsets[NB], on the device)
+    const uint32_t* so = pl.sorted.p + (size_t)view * bound;
     uint32_t rounds = 0;
     if (opts.batch_affine > 0 && bound >= ((uint64_t)1 << opts.batch_affine_min_log) && bound < (1ull << 31)) rounds = (uint32_t)opts.batch_affine;
     ws.tail_done.wait(st_);  // the previous proof's tail may still be reading these buffers
@@ -1139,16 +1169,31 @@ class Engine : public EngineBase {
     ws.acc_done.record(st_);
   }
 
+  // Levels of the device bucket reduction: it stops when a proof's windows hold at most host_nodes block totals, so the host
+  // share of every proof is the same whatever the batch size.  Returns the XYZZ entries of the result slot (all K proofs).
+  template <class F>
+  size_t tail_levels(const MsmPlan& pl, uint32_t& cnt, uint32_t& nbits) const {
+    const uint32_t Wp = pl.sh.pre ? 1 : pl.sh.W;
+    const uint32_t rbits = opts.bitsum_radix == 8 ? 3u : 1u;
+    // a G2 addition costs 1.3 us on a host core against 0.45 us in G1, and the G2 tail is never the last to finish:
+    // run it further down on the GPU
+    const size_t host_nodes = sizeof(F) > sizeof(Fq) ? HOST_TREE_NODES / 8 : HOST_TREE_NODES;
+    cnt = pl.sh.B; nbits = 0;
+    while (cnt >= (1u << rbits) && (size_t)Wp * cnt > host_nodes) { cnt >>= rbits; nbits += rbits; }
+    return (size_t)pl.sh.K * Wp * cnt * (1 + (size_t)nbits);
+  }
+
   // phase 2 (side stream): reduce chunk-boundary partials, then the bucket reduction by bit sums.  Latency-bound
   // (7 dependent point additions per level), so it runs on a high-priority stream underneath the next MSM's accumulation.
   template <class F>
-  void msm_tail(const MsmPlan& pl, MsmWs& ws, XYZZ<F>* win_out /* MAXW entries */, StageTimer* tm = nullptr, const char* tail_name = nullptr) {
+  void msm_tail(const MsmPlan& pl, MsmWs& ws, XYZZ<F>* win_out /* K * MAXW entries */, StageTimer* tm = nullptr, const char* tail_name = nullptr) {
     typedef XYZZ<F> X;
     if (pl.sh.n == 0) return;
     Stream ts = tail_stream(ws);
     ws.acc_done.wait(ts);
     size_t span = (tm && tail_name) ? tm->begin_on(ts, tail_name) : 0;
-    const uint32_t W = pl.sh.pre ? 1 : pl.sh.W, B = pl.sh.B, T2 = pl.T2, nt1 = ws.nt1;   // chunks of THIS accumulation
+    // the K bucket sets of a batch are K * W windows to the reduction kernels
+    const uint32_t W = (pl.sh.pre ? 1 : pl.sh.W) * pl.sh.K, B = pl.sh.B, T2 = pl.T2, nt1 = ws.nt1;   // chunks of THIS accumulation
     X* buckets = (X*)ws.buckets.p;
     uint32_t L = 2 * nt1;
     int cur = 0;
@@ -1175,11 +1220,9 @@ class Engine : public EngineBase {
       ws.tree[2].ensure((half + 1) * sizeof(X)); ws.tree[3].ensure((half + 1) * sizeof(X));
     }
     const X* inA = buckets; const X* inP = nullptr;
-    uint32_t cnt = B, lvl = 0, nbits = 0;
-    // a G2 addition costs 1.3 us on a host core against 0.45 us in G1, and the G2 tail is never the last to finish:
-    // run it further down on the GPU
-    const size_t host_nodes = sizeof(F) > sizeof(Fq) ? HOST_TREE_NODES / 8 : HOST_TREE_NODES;
-    while (cnt >= (1u << rbits) && (size_t)W * cnt > host_nodes) {
+    uint32_t cnt = B, lvl = 0, nbits = 0, end_cnt = 0, end_bits = 0;
+    const size_t out_entries = tail_levels<F>(pl, end_cnt, end_bits);
+    while (nbits < end_bits) {
       X* oA = (X*)ws.tree[lvl & 1].p; X* oP = (X*)ws.tree[2 + (lvl & 1)].p;
       const X* iA = inA; const X* iP = inP;
       const uint32_t ci = cnt, np = nbits;
@@ -1195,8 +1238,8 @@ class Engine : public EngineBase {
     // result slot: [A : W*cnt][pending 0 : W*cnt] ... [pending nbits-1 : W*cnt]; the host finishes (host_finish)
     ws.tree_cnt = cnt; ws.tree_bits = nbits;
     const size_t nodes = (size_t)W * cnt;
-    ws.out_entries = nodes * (1 + (size_t)nbits);
-    if (ws.out_entries > MAXW) throw Error(ZKB_E_INTERNAL, "msm result slot overflow");
+    ws.out_entries = out_entries;
+    if (ws.out_entries > (size_t)MAXW * pl.sh.K) throw Error(ZKB_E_INTERNAL, "msm result slot overflow");
     d2d(ts, win_out, inA, nodes * sizeof(X));
     if (nbits) d2d(ts, win_out + nodes, inP, nodes * nbits * sizeof(X));
     if (tm && tail_name) tm->end_on(ts, span);
@@ -1214,11 +1257,12 @@ class Engine : public EngineBase {
   //   sum_j (j + 1) B_j = total + sum_bit 2^bit S_bit + 2^nbits hi    (Horner from the top bit),
   // then result = sum_w 2^(c w) (window sum).  A few hundred point additions on a host core.
   static constexpr size_t HOST_TREE_NODES = 32;
+  // `proof`: which of the plan's K proofs (its windows are proof * W .. proof * W + W - 1 of every array of the slot)
   template <class HX>
-  static HX host_finish(const HX* slot, const MsmPlan& pl, const MsmWs& ws) {
+  static HX host_finish(const HX* slot, const MsmPlan& pl, const MsmWs& ws, uint32_t proof = 0) {
     const uint32_t W = pl.sh.pre ? 1 : pl.sh.W, cnt = ws.tree_cnt, nbits = ws.tree_bits, c = pl.sh.c;
-    const size_t nodes = (size_t)W * cnt;
-    const HX* A = slot;
+    const size_t nodes = (size_t)W * pl.sh.K * cnt, first = (size_t)proof * W * cnt;
+    const HX* A = slot + first;
     auto window_sum = [&](uint32_t w) {
       HX run = HX::identity(), hi = HX::identity();
       for (uint32_t k = cnt; k-- > 0;) {
@@ -1226,7 +1270,7 @@ class Engine : public EngineBase {
         if (k > 0) hi = HX::add(hi, run);
       }
       for (uint32_t bit = nbits; bit-- > 0;) {
-        const HX* P = slot + nodes * (1 + (size_t)bit) + (size_t)w * cnt;
+        const HX* P = slot + nodes * (1 + (size_t)bit) + first + (size_t)w * cnt;
         HX sb = HX::identity();
         for (uint32_t k = 0; k < cnt; k++) sb = HX::add(sb, P[k]);
         hi = HX::add(HX::dbl(hi), sb);
@@ -1707,7 +1751,7 @@ class Engine : public EngineBase {
     G1X* w_h = (G1X*)sl.d_win.p;
     {
       StreamScope sc(st_, wm_stream_);
-      wm_finish(r, sl, tm2);
+      wm_finish(r, sl.a.p, sl.b.p, sl.c.p, sl.h.p, 1, tm2, "witness_map_finish");
       tm2.begin("msm_plan_h");
       plan_build(sl.plan_h, sl.h.p + pk.hlo, pk.hhi - pk.hlo, 1, nullptr, pk.pre_ch);
       tm2.end();
@@ -1958,6 +2002,204 @@ class Engine : public EngineBase {
                   uint8_t* proof_out) override {
     const uint64_t t = prove_submit(pkh, rh, z, r, s);
     prove_collect(t, proof_out);
+  }
+
+  // ------------------------------------------------------------------------------ batch of proofs (zkb_groth16_prove_batch)
+  // K proofs of one circuit under one key share the key, its window tables, the matrices and the domain; only the
+  // assignments differ.  So a PASS of K proofs is one set of launches: one SpMV over all K assignments, transforms of all 3K
+  // chain vectors at once, and MSM plans with a batch dimension (K bucket sets keyed k * NB + bucket over the shared points,
+  // MsmShape).  The host tails of the K proofs (the last additions of each MSM, r / s multiples, final combination) run in
+  // parallel on host threads.
+  struct BatchState {
+    DevBuf<Fr> zc, zm, v, h;    // assignments (canonical, back to back; Montgomery, interleaved), 3K chains, K h vectors
+    MsmPlan plan_z, plan_h;
+    MsmWs ws[5];                // h, l, a, b1, b2
+    DevBuf<uint8_t> d_win;      // the K x 5 result slots, packed
+    HostBuf hw;
+    void destroy() { for (auto& w : ws) w.destroy(); }
+    size_t device_bytes() const {
+      size_t b = zc.bytes() + zm.bytes() + v.bytes() + h.bytes() + d_win.bytes();
+      for (const MsmPlan* p : {&plan_z, &plan_h})
+        b += p->digits.bytes() + p->ranks.bytes() + p->counts.bytes() + p->offsets.bytes() + p->sorted.bytes() + p->scan_tmp.bytes() +
+             p->view_tile_cnt.bytes() + p->view_tile_off.bytes() + p->view_pre32.bytes() + p->view_mask32.bytes();
+      for (const MsmWs& w : ws) {
+        b += w.buckets.bytes();
+        for (int k = 0; k < 2; k++) b += w.val[k].bytes() + w.key[k].bytes();
+        for (int k = 0; k < 4; k++) b += w.tree[k].bytes();
+      }
+      return b;
+    }
+  } batch_;
+  // From this domain size on a batch gains nothing over the two-slot pipeline (which overlaps the witness map with the MSMs
+  // and each proof's host tail with the next proof's kernels), so prove_batch drives the slots instead; so it does for a
+  // single proof.  Measured on H100: batches gain up to 2^17, break even at 2^18 and lose at 2^20 (DESIGN.md §7).
+  static constexpr uint32_t BATCH_SLOTS_MIN_LOG = 18;
+  static constexpr int SPMV_GROUP = 4;   // assignments per thread of the batched SpMV
+
+  // device bytes of one pass of K proofs (the buffers BatchState grows to), an upper estimate
+  size_t batch_bytes(const Pk& pk, const R1cs& rc, uint64_t K, uint32_t pre_c_z) const {
+    const uint64_t n = 1ull << rc.log_n;
+    size_t bytes = (size_t)K * (2 * rc.m + 4 * n) * FRB;
+    auto plan = [&](uint64_t cnt, uint32_t nviews, uint32_t pre_c, std::initializer_list<size_t> xs) -> size_t {
+      if (!cnt) return 0;
+      const uint32_t c = plan_c(cnt, pre_c), W = plan_w(c);
+      const uint64_t NB = K * (pre_c ? 1ull : W) << (c - 1), tot = K * cnt * W;
+      uint64_t T = (tot + opts.chunk_target - 1) / opts.chunk_target;
+      T = T < 8 ? 8 : T > 64 ? 64 : T;
+      const uint64_t nt1 = (tot + T - 1) / T;
+      size_t b = (size_t)tot * 4 * (2 + nviews) + (size_t)NB * 4 * (1 + nviews);
+      for (size_t x : xs) b += (size_t)NB * x * 11 / 4 + 2 * (2 * nt1 + 2) * (4 + x);   // buckets + reduction levels, partials
+      return b;
+    };
+    bytes += plan(pk.hi - pk.lo, 3, pre_c_z, {sizeof(G1X), sizeof(G1X), sizeof(G1X), sizeof(G2X)});
+    bytes += plan(pk.hhi - pk.hlo, 1, pk.pre_ch, {sizeof(G1X)});
+    return bytes;
+  }
+  // proofs per pass: the uint32 bound of the sorted lists, ZKB_OPT_BATCH_PASS_MAX, and what fits in free HBM
+  uint32_t batch_pass_size(const Pk& pk, const R1cs& rc, uint32_t K, uint32_t pre_c_z) {
+    uint64_t kmax = std::min<uint64_t>(plan_max_batch(pk.hi - pk.lo, 3, pre_c_z), plan_max_batch(pk.hhi - pk.hlo, 1, pk.pre_ch));
+    if (opts.batch_pass_max > 0) kmax = std::min<uint64_t>(kmax, (uint64_t)opts.batch_pass_max);
+    kmax = std::min<uint64_t>(kmax, K);
+    if (kmax == 0) throw Error(ZKB_E_ARG, "msm too large");
+#if !defined(ZKB_EMU)
+    size_t free_b = 0, total_b = 0;
+    ZKB_CUDA(cudaMemGetInfo(&free_b, &total_b));
+    const size_t reserve = (size_t)1 << 30, have = free_b + batch_.device_bytes();
+    const size_t avail = have > reserve ? have - reserve : 0;
+    for (size_t need = batch_bytes(pk, rc, kmax, pre_c_z); kmax > 1 && need > avail; need = batch_bytes(pk, rc, kmax, pre_c_z))
+      kmax = std::max<uint64_t>(1, std::min<uint64_t>(kmax - 1, (uint64_t)((double)kmax * avail / need)));
+#endif
+    return (uint32_t)kmax;
+  }
+
+  template <class Fn>
+  static void host_parallel(uint32_t count, Fn fn) {   // fn(k) for k < count on up to one host thread per core
+    uint32_t P = std::thread::hardware_concurrency();
+    P = std::max(1u, std::min(P ? P : 4u, count));
+    std::vector<std::future<void>> fs;
+    for (uint32_t q = 1; q < P; q++) fs.push_back(std::async(std::launch::async, [&fn, q, P, count] { for (uint32_t k = q; k < count; k += P) fn(k); }));
+    for (uint32_t k = 0; k < count; k += P) fn(k);
+    for (auto& f : fs) f.get();
+  }
+
+  void prove_batch(uint64_t pkh, uint64_t rh, uint32_t K, const uint64_t* z, const uint64_t* r, const uint64_t* s,
+                   uint8_t* proofs_out) override {
+    if (K == 0) throw Error(ZKB_E_ARG, "empty batch");
+    Pk& pk = get_pk(pkh);
+    R1cs& rc = get_r1cs(rh);
+    if (pk.m != rc.m || pk.ni != rc.ni) throw Error(ZKB_E_ARG, "proving key does not match the R1CS (variable counts)");
+    if (pk.hl + 1 != ((uint64_t)1 << rc.log_n)) throw Error(ZKB_E_ARG, "proving key does not match the R1CS (domain size)");
+    if (pk.world != 1) throw Error(ZKB_E_ARG, "a batch needs a key loaded whole (world = 1)");
+    for (auto& sl : slots_)
+      if (sl.state != 0) throw Error(ZKB_E_ARG, "a proof is in flight on this context (collect it first)");
+    const size_t zw = (size_t)rc.m * 4, pb = 8 * FQB;    // words per assignment, bytes per proof
+    if (rc.log_n >= BATCH_SLOTS_MIN_LOG || K == 1) {     // large circuits and single proofs: the two-slot pipeline
+      uint64_t prev = 0;
+      try {
+        for (uint32_t k = 0; k < K; k++) {
+          const uint64_t t = prove_submit(pkh, rh, z + k * zw, r + 4 * (size_t)k, s + 4 * (size_t)k);
+          if (k) prove_collect(prev, proofs_out + (k - 1) * pb);
+          prev = t;
+        }
+        prove_collect(prev, proofs_out + (K - 1) * pb);
+      } catch (...) {
+        std::vector<uint8_t> sink(pb);
+        for (auto& sl : slots_)
+          if (sl.state == 2) { try { prove_collect(sl.ticket, sink.data()); } catch (...) { sl.state = 0; } }
+        throw;
+      }
+      return;
+    }
+    // one z-MSM mode for the whole batch, from a sample of its assignments
+    uint32_t sampled = 0, sparse = 0;
+    for (uint32_t i = 0; i < std::min(K, 8u); i++, sampled++) sparse += assignment_is_sparse(z + (size_t)i * K / std::min(K, 8u) * zw, rc.m);
+    const uint32_t pre_c_z = z_window_mode(2 * sparse > sampled) ? 0 : pk.pre_cz;
+    const uint32_t kp = batch_pass_size(pk, rc, K, pre_c_z);
+    std::vector<std::pair<const char*, double>> all, part;
+    for (uint32_t k0 = 0; k0 < K; k0 += kp) {
+      const uint32_t cnt = std::min(kp, K - k0);
+      batch_pass(pk, rc, cnt, z + k0 * zw, r + 4 * (size_t)k0, s + 4 * (size_t)k0, pre_c_z, proofs_out + k0 * pb, part);
+      all.insert(all.end(), part.begin(), part.end());
+    }
+    timings = all;
+  }
+
+  void batch_pass(const Pk& pk, R1cs& rc, uint32_t K, const uint64_t* z, const uint64_t* r, const uint64_t* s, uint32_t pre_c_z,
+                  uint8_t* proofs_out, std::vector<std::pair<const char*, double>>& times) {
+    BatchState& b = batch_;
+    DomainT& d = domain(rc.log_n);
+    const uint32_t lg = rc.log_n;
+    const size_t n = (size_t)1 << lg, m = rc.m;
+    // r * d1, s * d1, rs * d1 and s * d2 need nothing from the GPU: host threads compute them underneath the kernels
+    std::vector<FixedMults> fms(K);
+    std::future<void> fm_all = std::async(std::launch::async, [&] {
+      host_parallel(K, [&](uint32_t k) { fms[k] = fixed_mults(pk, (const uint32_t*)(r + 4 * (size_t)k), (const uint32_t*)(s + 4 * (size_t)k)); });
+    });
+    b.zc.ensure(K * m); b.zm.ensure(K * m); b.v.ensure(3 * K * n); b.h.ensure(K * n);
+    StageTimer tm(st_);
+    tm.begin("h2d_z_batch");
+    h2d(st_, b.zc.p, z, K * m * FRB);
+    tm.end();
+    tm.begin("witness_map_batch");
+    {
+      const Fr* zc = b.zc.p; Fr* zm = b.zm.p;
+      launch<k_fr_convert>(st_, K * m, ZKB_LAMBDA(size_t t) { zm[(t % m) * K + t / m] = Fr::to_mont(zc[t]); });
+      const uint32_t* rpA = rc.rowptr[0].p; const uint32_t* clA = rc.col[0].p; const Fr* vlA = rc.val[0].p;
+      const uint32_t* rpB = rc.rowptr[1].p; const uint32_t* clB = rc.col[1].p; const Fr* vlB = rc.val[1].p;
+      const uint32_t* rpC = rc.rowptr[2].p; const uint32_t* clC = rc.col[2].p; const Fr* vlC = rc.val[2].p;
+      Fr* v = b.v.p;
+      const uint32_t N = (uint32_t)rc.N, ni = (uint32_t)rc.ni, ngroups = (K + SPMV_GROUP - 1) / SPMV_GROUP;
+      // thread (matrix, group of assignments, row): the row index runs fastest, so the output stores are coalesced
+      launch<k_spmv>(st_, 3 * (size_t)ngroups * n, ZKB_LAMBDA(size_t t) {
+        const uint32_t row = (uint32_t)(t & (n - 1)), q = (uint32_t)(t >> lg), kind = q / ngroups, g = q % ngroups;
+        const uint32_t* rp = kind == 0 ? rpA : kind == 1 ? rpB : rpC;
+        const uint32_t* cl = kind == 0 ? clA : kind == 1 ? clB : clC;
+        const Fr* vl = kind == 0 ? vlA : kind == 1 ? vlB : vlC;
+        spmv_batch_body<Fr, SPMV_GROUP>(rp, cl, vl, zm, K, g * SPMV_GROUP, v + (size_t)kind * K * n, n, N, kind == 0 ? ni : 0, row);
+      });
+      ntt_dif(v, d.tw_inv.p, lg, 3 * K);
+      ntt_dit(v, d.tw_fwd.p, lg, d.cos_fwd.p, 3 * K);   // coset shift fused into the first pass, as in wm_chains
+      wm_finish(rc, v, v + K * n, v + 2 * K * n, b.h.p, K, tm, "witness_map_finish_batch");
+    }
+    tm.end();
+    tm.begin("msm_plan_z_batch");
+    plan_build(b.plan_z, b.zc.p + 1 + pk.lo, pk.hi - pk.lo, 3, pk.skip.p, pre_c_z, K, m);
+    tm.end();
+    tm.begin("msm_plan_h_batch");
+    plan_build(b.plan_h, b.h.p + pk.hlo, pk.hhi - pk.hlo, 1, nullptr, pk.pre_ch, K, n);
+    tm.end();
+    // result slots of the five MSMs (h, l, a, b1: G1; b2: G2), packed so that one copy brings all of them to the host
+    uint32_t tc, tb;
+    const size_t ez = b.plan_z.sh.n ? tail_levels<Fq>(b.plan_z, tc, tb) : 0, ez2 = b.plan_z.sh.n ? tail_levels<Fq2>(b.plan_z, tc, tb) : 0;
+    const size_t eh = b.plan_h.sh.n ? tail_levels<Fq>(b.plan_h, tc, tb) : 0;
+    const size_t off[6] = {0, eh * sizeof(G1X), (eh + ez) * sizeof(G1X), (eh + 2 * ez) * sizeof(G1X), (eh + 3 * ez) * sizeof(G1X),
+                           (eh + 3 * ez) * sizeof(G1X) + ez2 * sizeof(G2X)};
+    b.d_win.ensure(off[5]);
+    b.hw.ensure(off[5]);
+    uint8_t* dw = b.d_win.p;
+    msm_exec<Fq2>(b.plan_z, pk.b2.p, (G2X*)(dw + off[4]), b.ws[4], &tm, "accum1_g2_b2_batch", 2, "tail_g2_b2_batch");
+    msm_exec<Fq>(b.plan_z, pk.l.p, (G1X*)(dw + off[1]), b.ws[1], &tm, "accum1_g1_l_batch", 0, "tail_g1_l_batch");
+    msm_exec<Fq>(b.plan_z, pk.a.p, (G1X*)(dw + off[2]), b.ws[2], &tm, "accum1_g1_a_batch", 1, "tail_g1_a_batch");
+    msm_exec<Fq>(b.plan_z, pk.b1.p, (G1X*)(dw + off[3]), b.ws[3], &tm, "accum1_g1_b1_batch", 2, "tail_g1_b1_batch");
+    msm_exec<Fq>(b.plan_h, pk.h.p, (G1X*)(dw + off[0]), b.ws[0], &tm, "accum1_g1_h_batch", 0, "tail_g1_h_batch");
+    for (auto& w : b.ws) w.tail_done.wait(st_);
+    tm.begin("d2h_windows_batch");
+    d2h(st_, b.hw.p, dw, off[5]);
+    tm.end();
+    stream_sync(st_);
+    tm.collect(times);
+    fm_all.get();
+    const auto t0 = std::chrono::steady_clock::now();
+    const uint8_t* hw = b.hw.p;
+    host_parallel(K, [&](uint32_t k) {
+      HostPartial hp;
+      auto g1 = [&](int slot, const MsmPlan& pl) { return pl.sh.n ? host_finish<HG1X>((const HG1X*)(hw + off[slot]), pl, b.ws[slot], k) : HG1X::identity(); };
+      hp.h = g1(0, b.plan_h); hp.l = g1(1, b.plan_z); hp.a = g1(2, b.plan_z); hp.b1 = g1(3, b.plan_z);
+      hp.b2 = b.plan_z.sh.n ? host_finish<HG2X>((const HG2X*)(hw + off[4]), b.plan_z, b.ws[4], k) : HG2X::identity();
+      finalize_with(pk, fms[k], (const uint8_t*)&hp, 1, (const uint32_t*)(r + 4 * (size_t)k), (const uint32_t*)(s + 4 * (size_t)k),
+                    proofs_out + (size_t)k * 8 * FQB);
+    });
+    times.push_back({"host_tails_batch", std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count()});
   }
 
   // ------------------------------------------------------------------------------ standalone MSM (tests / microbench)

@@ -25,6 +25,7 @@ struct Options {
   int64_t ntt_kernel = 2;     // ZKB_OPT_NTT_KERNEL: 2 = four-step twiddles / cp.async tile load (ntt_tile.cuh), 1 = the round-1 tile pass
   int64_t pk_cache = 1;       // ZKB_OPT_PK_CACHE: share proving keys by content and keep the last released one resident
   int64_t bitsum_radix = 2;   // ZKB_OPT_BITSUM_RADIX: bucket-reduction levels of radix 2 (1 dependent addition per launch) or 8 (7)
+  int64_t batch_pass_max = 0; // ZKB_OPT_BATCH_PASS_MAX: most proofs of zkb_groth16_prove_batch per pass; 0 = as many as fit in HBM
 };
 
 struct EngineBase {
@@ -56,6 +57,8 @@ struct EngineBase {
                         uint8_t* proof_out) = 0;
   virtual void prove_full(uint64_t pk, uint64_t r1cs, const uint64_t* z, const uint64_t* r, const uint64_t* s,
                           uint8_t* proof_out) = 0;
+  virtual void prove_batch(uint64_t pk, uint64_t r1cs, uint32_t count, const uint64_t* z, const uint64_t* r, const uint64_t* s,
+                           uint8_t* proofs_out) = 0;
   virtual void msm(int group, const uint8_t* points, const uint64_t* scalars, uint64_t n, uint8_t* out) = 0;
   virtual void ntt(uint64_t* data, uint32_t log_n, int inverse, int coset) = 0;
   virtual void witness_map(uint64_t r1cs, const uint64_t* z, uint64_t* h_out, uint64_t cap) = 0;
@@ -68,6 +71,7 @@ struct EngineBase {
                                         size_t cap, size_t* wit_len) = 0;
   virtual void prog_set_witness(uint64_t h, const uint8_t* wit, size_t len) = 0;
   virtual uint64_t prog_public_inputs(uint64_t h, uint64_t* out, uint64_t cap) = 0;
+  virtual void prog_assignment(uint64_t h, uint64_t* z_out, uint64_t cap_elems) = 0;
   virtual void field_op(int field, int op, const uint64_t* a, const uint64_t* b, uint64_t* out, uint64_t n) = 0;
   virtual uint64_t gm17_pk_load(const uint8_t* pk, size_t len) = 0;
   virtual void gm17_pk_free(uint64_t h) = 0;

@@ -32,14 +32,19 @@ __device__ __forceinline__ uint32_t zkb_atomic_add(uint32_t* p, uint32_t v) { re
 inline uint32_t zkb_atomic_add(uint32_t* p, uint32_t v) { uint32_t o = *p; *p = o + v; return o; }
 #endif
 
+// A plan may carry a BATCH of K scalar vectors over the same n points (K proofs of one circuit): every proof has its own
+// bucket set, bucket key k * NB + bucket with NB = msm_set_buckets, while the sorted entries still name the shared point
+// (or its table entry w * n + i).  The accumulate and reduction kernels only see K * NB buckets and K * W windows.
 struct MsmShape {
-  uint32_t n;        // number of (scalar, point) pairs
+  uint32_t n;        // number of (scalar, point) pairs of one proof
   uint32_t c;        // window bits
   uint32_t W;        // windows
   uint32_t B;        // buckets per window = 2^(c-1)
   uint32_t pre;      // 1: the point table holds 2^(c w) P_i at index w*n + i, so all windows share ONE bucket set
+  uint32_t K;        // scalar vectors (proofs) in the batch, >= 1
 };
-ZKB_HD uint32_t msm_nbuckets(const MsmShape& sh) { return sh.pre ? sh.B : sh.W * sh.B; }
+ZKB_HD uint32_t msm_set_buckets(const MsmShape& sh) { return sh.pre ? sh.B : sh.W * sh.B; }
+ZKB_HD uint32_t msm_nbuckets(const MsmShape& sh) { return sh.K * msm_set_buckets(sh); }
 
 ZKB_HD uint32_t scalar_bits(const uint32_t* s, uint32_t lo, uint32_t cnt) {
   // bits [lo, lo+cnt) of a 256-bit little-endian scalar, cnt <= 31
@@ -49,17 +54,22 @@ ZKB_HD uint32_t scalar_bits(const uint32_t* s, uint32_t lo, uint32_t cnt) {
   return (uint32_t)(v >> sh) & ((1u << cnt) - 1u);
 }
 
-// ---- digits + histogram: one thread per scalar -------------------------------------------------
-// digits[w * n + i] = (|d| - 1) | sign, or MSM_NONE when d == 0;  ranks[w * n + i] = arrival order of the entry inside its
-// bucket (the value the histogram atomic returned), so the scatter needs no second atomic.
-ZKB_HDN inline void msm_digits_body(MsmShape sh, const uint32_t* scalars /* n x 8, canonical */, uint32_t* digits, uint32_t* ranks,
-                                    uint32_t* counts /* W*B (or B with tables) */, uint32_t i) {
-  if (i >= sh.n) return;
+// ---- digits + histogram: one thread per (proof, scalar) ---------------------------------------
+// Scalar vector k starts at scalars + k * stride elements.  digits[(k W + w) n + i] = (|d| - 1) | sign, or MSM_NONE when
+// d == 0;  ranks[.] = arrival order of the entry inside its bucket (the value the histogram atomic returned), so the scatter
+// needs no second atomic.  The plan keeps K n W < 2^32 (engine.cuh::plan_build), so thread indices divide in 32 bits.
+ZKB_HDN inline void msm_digits_body(MsmShape sh, const uint32_t* scalars /* canonical, 8 words each */, size_t stride, uint32_t* digits,
+                                    uint32_t* ranks, uint32_t* counts /* K * msm_set_buckets */, uint32_t t) {
+  if (t >= sh.K * sh.n) return;
+  const uint32_t k = t / sh.n, i = t % sh.n;
+  const uint32_t* src = scalars + ((size_t)k * stride + i) * 8;
   uint32_t s[8];
 #pragma unroll
-  for (int k = 0; k < 8; k++) s[k] = scalars[(size_t)i * 8 + k];
+  for (int q = 0; q < 8; q++) s[q] = src[q];
   uint32_t carry = 0;
   const uint32_t full = 1u << sh.c, half = sh.B;
+  const uint32_t kbase = k * msm_set_buckets(sh);
+  const size_t row0 = (size_t)k * sh.W;
   for (uint32_t w = 0; w < sh.W; w++) {
     uint32_t d = scalar_bits(s, w * sh.c, sh.c) + carry;
     uint32_t code;
@@ -76,24 +86,24 @@ ZKB_HDN inline void msm_digits_body(MsmShape sh, const uint32_t* scalars /* n x 
       code = d - 1;
       carry = 0;
     }
-    digits[(size_t)w * sh.n + i] = code;
+    const size_t slot = (row0 + w) * sh.n + i;
+    digits[slot] = code;
     if (code != MSM_NONE) {
-      const uint32_t key = (sh.pre ? 0u : w * sh.B) + (code & ~MSM_NEG);
-      ranks[(size_t)w * sh.n + i] = zkb_atomic_add(&counts[key], 1);
+      const uint32_t key = kbase + (sh.pre ? 0u : w * sh.B) + (code & ~MSM_NEG);
+      ranks[slot] = zkb_atomic_add(&counts[key], 1);
     }
   }
 }
 
-// ---- scatter: one thread per (window, scalar) --------------------------------------------------
+// ---- scatter: one thread per (proof, window, scalar) ----------------------------------------------
 // sorted[offsets[key] + rank] = point index | sign      (counting sort; the order inside a bucket is irrelevant: sums)
 ZKB_HDN inline void msm_scatter_body(MsmShape sh, const uint32_t* digits, const uint32_t* ranks, const uint32_t* offsets,
-                                     uint32_t* sorted, size_t t) {
-  const size_t total = (size_t)sh.n * sh.W;
-  if (t >= total) return;
+                                     uint32_t* sorted, uint32_t t) {
+  if (t >= sh.K * sh.n * sh.W) return;
   uint32_t code = digits[t];
   if (code == MSM_NONE) return;
-  uint32_t w = (uint32_t)(t / sh.n), i = (uint32_t)(t % sh.n);
-  uint32_t key = (sh.pre ? 0u : w * sh.B) + (code & ~MSM_NEG);
+  const uint32_t kw = t / sh.n, i = t % sh.n, w = kw % sh.W, k = kw / sh.W;
+  uint32_t key = k * msm_set_buckets(sh) + (sh.pre ? 0u : w * sh.B) + (code & ~MSM_NEG);
   const uint32_t val = (sh.pre ? w * sh.n + i : i) | (code & MSM_NEG);
   sorted[offsets[key] + ranks[t]] = val;
 }

@@ -267,6 +267,36 @@ ZKB_HDN inline void spmv_body(const uint32_t* rowptr, const uint32_t* col, const
   out[t] = acc;
 }
 
+// The same product for a batch of K assignments, G of them per thread: one thread reads a CSR row (columns and
+// coefficients) once and accumulates G dot products.  z is INTERLEAVED, z[col * K + k]: the G values a term needs sit in
+// G * 32 consecutive bytes (one or two cache lines) instead of G lines K * m * 32 bytes apart.  Vector k of the output
+// starts at out + k * n (rows 0 .. n - 1 of the domain): rows below n_rows hold the products, the next n_copy rows
+// z[row - n_rows] (the instance variables of the A chain, n_copy = 0 for B and C), the rest zero.
+template <class Fr, int G>
+ZKB_HDN inline void spmv_batch_body(const uint32_t* rowptr, const uint32_t* col, const Fr* val, const Fr* z, uint32_t K, uint32_t k0,
+                                    Fr* out, size_t n, uint32_t n_rows, uint32_t n_copy, uint32_t row) {
+  const uint32_t kn = K - k0 < (uint32_t)G ? K - k0 : (uint32_t)G;
+  Fr acc[G];
+#pragma unroll
+  for (int g = 0; g < G; g++) acc[g] = Fr::zero();
+  if (row < n_rows) {
+    for (uint32_t e = rowptr[row]; e < rowptr[row + 1]; e++) {
+      const Fr v = val[e];
+      const Fr* zr = z + (size_t)col[e] * K + k0;
+#pragma unroll
+      for (int g = 0; g < G; g++)
+        if ((uint32_t)g < kn) acc[g] = Fr::add(acc[g], Fr::mul(v, zr[g]));
+    }
+  } else if (row - n_rows < n_copy) {
+#pragma unroll
+    for (int g = 0; g < G; g++)
+      if ((uint32_t)g < kn) acc[g] = z[(size_t)(row - n_rows) * K + k0 + g];
+  }
+#pragma unroll
+  for (int g = 0; g < G; g++)
+    if ((uint32_t)g < kn) out[(size_t)(k0 + g) * n + row] = acc[g];
+}
+
 
 // ---- levelised witness evaluation / R1CS satisfaction check ------------------------------------------------
 // Restates the per-statement rule of zokrates_interpreter/src/lib.rs:61-138 on the R1CS rows: a constraint whose linear side

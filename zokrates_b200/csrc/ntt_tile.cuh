@@ -159,8 +159,9 @@ __device__ __forceinline__ void ntt2_stages(Fr* __restrict__ x, const Fr* __rest
   }
 }
 
+// `tiles` counts the tiles of all vectors: a batch of vectors of 2^log_n elements back to back shares the twiddles
 template <class Fr, bool DIT>
-__global__ void __launch_bounds__(NTT_BLOCK, 4) zkb_ntt_tile2(Fr* x, const Fr* tw, const Fr* scale, NttPass ps, uint32_t tiles) {
+__global__ void __launch_bounds__(NTT_BLOCK, 4) zkb_ntt_tile2(Fr* x_all, const Fr* tw, const Fr* scale, NttPass ps, uint32_t tiles) {
   extern __shared__ uint4 ntt2_smem[];
   uint4* dlo = ntt2_smem;
   uint4* dhi = dlo + NTT2_PLANE;
@@ -175,7 +176,10 @@ __global__ void __launch_bounds__(NTT_BLOCK, 4) zkb_ntt_tile2(Fr* x, const Fr* t
       whi[ntt2_wslot(k)] = src[1];
     }
   }
-  for (uint32_t tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+  const uint32_t lg_tpv = ps.log_n - NTT_TILE_LOG;                    // tiles per vector: 2^lg_tpv
+  for (uint32_t bt = blockIdx.x; bt < tiles; bt += gridDim.x) {
+    Fr* x = x_all + ((size_t)(bt >> lg_tpv) << ps.log_n);
+    const uint32_t tile = bt & ((1u << lg_tpv) - 1u);
     __syncthreads();                       // the previous tile's last phase has read its shared data
     for (uint32_t k = 0; k < NTT_TILE / NTT_BLOCK; k++) {
       const uint32_t e = threadIdx.x + k * NTT_BLOCK;
