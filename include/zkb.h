@@ -100,9 +100,10 @@ int32_t zkb_pk_table_info(zkb_ctx* ctx, uint64_t pk_handle, uint64_t out[8]);
                                  * query vector at zkb_pk_load; -1 (default) from a cost model, 0 equal shares, > 0 the chain's cost in
                                  * 1/1000 of the whole MSM work.  Must be equal on all ranks (the cuts are derived independently). */
 #define ZKB_OPT_NTT_KERNEL 9    /* tile pass of the NTT: 2 (default) four-step twiddles + cp.async tile load, 1 the round-1 pass */
-#define ZKB_OPT_BATCH_PASS_MAX 15 /* most proofs zkb_groth16_prove_batch runs as one pass (one set of launches); 0 (default) = as many as
+#define ZKB_OPT_BATCH_PASS_MAX 15 /* most proofs zkb_groth16_prove_batch / zkb_prog_prove_batch, and most input sets
+                                   * zkb_prog_compute_witness_batch, run as one pass (one set of launches); 0 (default) = as many as
                                    * fit in free HBM and in the 32-bit indices of the sorted MSM lists.  Larger batches run as several
-                                   * passes with the same proofs; tests use it to force several passes */
+                                   * passes with the same results; tests use it to force several passes */
 #define ZKB_OPT_PK_CACHE 8      /* 1 (default): zkb_pk_load of bytes that are already resident returns a handle onto the same key
                                  * (content fingerprint), and the last key released by zkb_pk_free stays resident until another
                                  * key is loaded — the per-call pk_load / prove / pk_free of the static trait method then builds
@@ -244,6 +245,30 @@ int32_t zkb_prog_free(zkb_ctx* ctx, uint64_t prog_handle);
 int32_t zkb_prog_compute_witness(zkb_ctx* ctx, uint64_t prog_handle, const uint64_t* inputs, uint64_t n_inputs, uint32_t flags,
                                  uint8_t* witness_out, size_t witness_cap, size_t* witness_len, uint64_t* first_unsatisfied);
 int32_t zkb_prog_set_witness(zkb_ctx* ctx, uint64_t prog_handle, const uint8_t* witness_bytes, size_t len);
+
+/* Batches of input sets of one program.  inputs: count sets of n_inputs canonical elements back to back; flags as in
+ * zkb_prog_compute_witness, for every set.  One level sweep serves all sets: the launch count does not grow with count.
+ * first_unsatisfied[count]: set k's first violated constraint (the index zkb_prog_compute_witness reports for the same
+ * inputs), UINT64_MAX when it is satisfied.  When some set fails the call returns ZKB_E_UNSAT; every other set's results are
+ * complete and the failing sets' output slots are zero-filled.  Refused as a whole, before any launch, with the codes of the
+ * single call: count 0, a wrong n_inputs, a non-canonical input in any set, a program that cannot be scheduled or calls a
+ * solver without a device path, a short buffer.  Neither call changes the program's resident assignment (what
+ * zkb_prog_public_inputs, zkb_prog_assignment and zkb_groth16_prove_resident read).
+ * zkb_prog_compute_witness_batch: witness_out (may be NULL) receives count witness FILES back to back, all of one length
+ *   *witness_len (8 + 40 x defined variables), file k byte-identical to zkb_prog_compute_witness on set k.
+ * zkb_prog_prove_batch: inputs -> count Groth16 proofs under pk_handle, the assignments never leaving the device below a 2^18
+ *   domain (the witness sweep writes the batched prover's interleaved assignment; from 2^18 on, and for count 1, the proofs
+ *   run through the two-slot pipeline as in zkb_groth16_prove_batch).  r, s: count scalars each; proofs_out: count x
+ *   zkb_curve_sizes()[2] bytes, proof k byte-identical to zkb_prog_compute_witness on set k + zkb_groth16_prove_resident
+ *   with (r_k, s_k).  public_out (may be NULL): count x (public inputs) elements, set k's in the order of
+ *   zkb_prog_public_inputs; public_cap counts elements.  Further ZKB_E_ARG refusals are zkb_groth16_prove_batch's: a key
+ *   loaded with world > 1, a proof in flight (it stays collectable), a key that does not match the program's R1CS. */
+int32_t zkb_prog_compute_witness_batch(zkb_ctx* ctx, uint64_t prog_handle, uint32_t count, const uint64_t* inputs, uint64_t n_inputs,
+                                       uint32_t flags, uint8_t* witness_out, size_t witness_cap, size_t* witness_len,
+                                       uint64_t* first_unsatisfied);
+int32_t zkb_prog_prove_batch(zkb_ctx* ctx, uint64_t prog_handle, uint64_t pk_handle, uint32_t count, const uint64_t* inputs,
+                             uint64_t n_inputs, uint32_t flags, const uint64_t* r, const uint64_t* s, uint8_t* proofs_out,
+                             size_t proofs_cap, uint64_t* public_out, uint64_t public_cap, uint64_t* first_unsatisfied);
 int32_t zkb_prog_public_inputs(zkb_ctx* ctx, uint64_t prog_handle, uint64_t* out, uint64_t cap, uint64_t* count);
 int32_t zkb_prog_assignment(zkb_ctx* ctx, uint64_t prog_handle, uint64_t* z_out, uint64_t cap_elems);
 

@@ -31,7 +31,7 @@ SYMBOLS = [
     "zkb_groth16_prove_chains_to_stream", "zkb_groth16_prove_stream_to_finish",
     "zkb_prog_load", "zkb_prog_info", "zkb_prog_free", "zkb_prog_compute_witness", "zkb_prog_set_witness",
     "zkb_prog_public_inputs", "zkb_gm17_pk_load", "zkb_gm17_pk_free", "zkb_gm17_prove", "zkb_gm17_setup", "zkb_gm17_setup_size",
-    "zkb_groth16_prove_batch", "zkb_prog_assignment",
+    "zkb_groth16_prove_batch", "zkb_prog_assignment", "zkb_prog_compute_witness_batch", "zkb_prog_prove_batch",
 ]
 
 OPT_TABLES, OPT_TABLE_MIN_LOG, OPT_TABLE_C, OPT_Z_MODE, OPT_NTT_TILE_MIN, OPT_NTT_MAX_S, OPT_BITSUM_RADIX, OPT_PK_CACHE, OPT_NTT_KERNEL, OPT_BATCH_AFFINE, OPT_BATCH_AFFINE_MIN_LOG = 1, 2, 3, 4, 5, 6, 7, 8, 9, 10, 11
@@ -112,6 +112,10 @@ class Library:
         d.zkb_prog_free.argtypes = [C.c_void_p, C.c_uint64]
         d.zkb_prog_compute_witness.argtypes = [C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64, C.c_uint32, C.c_void_p, C.c_size_t,
                                                C.POINTER(C.c_size_t), _u64p]
+        d.zkb_prog_compute_witness_batch.argtypes = [C.c_void_p, C.c_uint64, C.c_uint32, C.c_void_p, C.c_uint64, C.c_uint32,
+                                                     C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t), C.c_void_p]
+        d.zkb_prog_prove_batch.argtypes = [C.c_void_p, C.c_uint64, C.c_uint64, C.c_uint32, C.c_void_p, C.c_uint64, C.c_uint32,
+                                           C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_uint64, C.c_void_p]
         d.zkb_prog_set_witness.argtypes = [C.c_void_p, C.c_uint64, C.c_void_p, C.c_size_t]
         d.zkb_prog_public_inputs.argtypes = [C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64, _u64p]
         d.zkb_msm_g1.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p]
@@ -410,6 +414,66 @@ class Context:
         self.lib.check(self.lib.dll.zkb_prog_compute_witness(self.h, prog, arr.ctypes.data if len(arr) else None, len(arr),
                                                              1 if try_out_of_range else 0, out.ctypes.data, cap, C.byref(n), C.byref(first)))
         return out[:n.value].tobytes()
+
+    def _input_sets(self, prog: int, inputs_list):
+        """K input sets -> (K, n, 4) uint64 array; every set must have the program's argument count (else the library refuses)"""
+        n = len(inputs_list[0]) if len(inputs_list) else 0
+        if any(len(x) != n for x in inputs_list):
+            raise ValueError("all input sets must have the same length")
+        arr = np.zeros((len(inputs_list), n, 4), dtype=np.uint64)
+        for k, x in enumerate(inputs_list):
+            if n:
+                arr[k] = fr_array([int(v) for v in x])
+        return arr, n
+
+    def prog_compute_witness_batch(self, prog: int, inputs_list, try_out_of_range: bool = False):
+        """K input sets in one level sweep (zkb_prog_compute_witness_batch).  Returns (witnesses, first_unsatisfied): entry k is
+        set k's witness FILE bytes and None, or None and the index of its first violated constraint."""
+        arr, n = self._input_sets(prog, inputs_list)
+        k = len(inputs_list)
+        info = self.prog_info(prog)
+        cap = 8 + 40 * (info["instance"] + info["witness"] + info["extra_variables"])
+        out = np.zeros(max(k, 1) * cap, dtype=np.uint8)
+        ln = C.c_size_t(0)
+        first = np.zeros(max(k, 1), dtype=np.uint64)
+        st = self.lib.dll.zkb_prog_compute_witness_batch(self.h, prog, k, arr.ctypes.data if arr.size else None, n,
+                                                         1 if try_out_of_range else 0, out.ctypes.data, k * cap, C.byref(ln),
+                                                         first.ctypes.data)
+        if st != 5:
+            self.lib.check(st)
+        size = ln.value
+        sat = [int(f) == (1 << 64) - 1 for f in first[:k]]
+        return ([out[i * size:(i + 1) * size].tobytes() if sat[i] else None for i in range(k)],
+                [None if sat[i] else int(first[i]) for i in range(k)])
+
+    def prog_prove_batch(self, prog: int, pk: int, inputs_list, rs, ss, try_out_of_range: bool = False):
+        """Inputs -> K proofs (zkb_prog_prove_batch), the assignments resident on the device.  Returns (proofs,
+        first_unsatisfied): entry k is (proof bytes, public inputs) and None, or None and set k's first violated constraint.
+        Proof k equals prog_compute_witness(prog, inputs_list[k]) + prove_resident(pk, r1cs, rs[k], ss[k])."""
+        arr, n = self._input_sets(prog, inputs_list)
+        k = len(inputs_list)
+        if len(rs) != k or len(ss) != k:
+            raise ValueError("inputs_list, rs and ss must have the same length")
+        info = self.prog_info(prog)
+        npub = info["public_arguments"] + info["returns"]
+        ra, sa = fr_array(list(rs)), fr_array(list(ss))
+        out = np.zeros(max(k, 1) * self.proof_bytes, dtype=np.uint8)
+        pub = np.zeros((max(k * npub, 1), 4), dtype=np.uint64)
+        first = np.zeros(max(k, 1), dtype=np.uint64)
+        st = self.lib.dll.zkb_prog_prove_batch(self.h, prog, pk, k, arr.ctypes.data if arr.size else None, n,
+                                               1 if try_out_of_range else 0, ra.ctypes.data, sa.ctypes.data, out.ctypes.data,
+                                               k * self.proof_bytes, pub.ctypes.data, k * npub, first.ctypes.data)
+        if st != 5:
+            self.lib.check(st)
+        res, bad = [], []
+        for i in range(k):
+            if int(first[i]) == (1 << 64) - 1:
+                res.append((out[i * self.proof_bytes:(i + 1) * self.proof_bytes].tobytes(), fr_from_array(pub[i * npub:(i + 1) * npub]) if npub else []))
+                bad.append(None)
+            else:
+                res.append(None)
+                bad.append(int(first[i]))
+        return res, bad
 
     def prog_set_witness(self, prog: int, witness_bytes: bytes):
         buf = np.frombuffer(witness_bytes, dtype=np.uint8)

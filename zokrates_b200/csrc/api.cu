@@ -360,6 +360,28 @@ int32_t zkb_prog_compute_witness(zkb_ctx* ctx, uint64_t h, const uint64_t* input
     if (f != ~0ull) throw Error(ZKB_E_UNSAT, "constraint " + std::to_string(f) + " is not satisfied");
   });
 }
+int32_t zkb_prog_compute_witness_batch(zkb_ctx* ctx, uint64_t h, uint32_t count, const uint64_t* inputs, uint64_t n_inputs,
+                                       uint32_t flags, uint8_t* witness_out, size_t witness_cap, size_t* witness_len,
+                                       uint64_t* first_unsatisfied) {
+  return guard(ctx, [&] {
+    if ((!inputs && n_inputs && count) || !first_unsatisfied) throw Error(ZKB_E_ARG, "null argument");
+    if (!ctx->eng->prog_compute_witness_batch(h, count, inputs, n_inputs, flags, witness_out, witness_cap, witness_len, first_unsatisfied))
+      throw Error(ZKB_E_UNSAT, "an input set does not satisfy the constraints (see first_unsatisfied)");
+  });
+}
+int32_t zkb_prog_prove_batch(zkb_ctx* ctx, uint64_t prog_handle, uint64_t pk_handle, uint32_t count, const uint64_t* inputs,
+                             uint64_t n_inputs, uint32_t flags, const uint64_t* r, const uint64_t* s, uint8_t* proofs_out,
+                             size_t proofs_cap, uint64_t* public_out, uint64_t public_cap, uint64_t* first_unsatisfied) {
+  return guard(ctx, [&] {
+    if ((!inputs && n_inputs && count) || !r || !s || !proofs_out || !first_unsatisfied) throw Error(ZKB_E_ARG, "null argument");
+    uint64_t sz[4];
+    ctx->eng->sizes(sz);
+    if (proofs_cap < (size_t)count * sz[2]) throw Error(ZKB_E_ARG, "proof buffer too small");
+    if (!ctx->eng->prog_prove_batch(prog_handle, pk_handle, count, inputs, n_inputs, flags, r, s, proofs_out, public_out, public_cap,
+                                    first_unsatisfied))
+      throw Error(ZKB_E_UNSAT, "an input set does not satisfy the constraints (see first_unsatisfied)");
+  });
+}
 int32_t zkb_prog_set_witness(zkb_ctx* ctx, uint64_t h, const uint8_t* witness_bytes, size_t len) {
   return guard(ctx, [&] {
     if (!witness_bytes) throw Error(ZKB_E_ARG, "null argument");

@@ -739,7 +739,7 @@ class Engine : public EngineBase {
       const uint32_t* nul = nullptr;
       const uint32_t N = (uint32_t)r.N;
       launch<k_witness_level>(st_, r.N, ZKB_LAMBDA(size_t t) {
-        witness_level_body<Fr>(rpA, clA, vlA, rpB, clB, vlB, rpC, clC, vlC, zm, nul, nul, 0, N, flag, (uint32_t)t);
+        witness_level_body<Fr>(rpA, clA, vlA, rpB, clB, vlB, rpC, clC, vlC, zm, nul, nul, 0, N, 1u, flag, (uint32_t)t);
       });
     } else {
       if (!level_ptr || !rows || !out_var) throw Error(ZKB_E_ARG, "null level description");
@@ -755,7 +755,7 @@ class Engine : public EngineBase {
       for (uint32_t l = 0; l < n_levels; l++) {
         const uint32_t lo = level_ptr[l], hi = level_ptr[l + 1];
         launch<k_witness_level>(st_, hi - lo, ZKB_LAMBDA(size_t t) {
-          witness_level_body<Fr>(rpA, clA, vlA, rpB, clB, vlB, rpC, clC, vlC, zm, pr, po, lo, hi, flag, (uint32_t)t);
+          witness_level_body<Fr>(rpA, clA, vlA, rpB, clB, vlB, rpC, clC, vlC, zm, pr, po, lo, hi, 1u, flag, (uint32_t)t);
         });
       }
       convert(r.z_mont.p, r.z_canon.p, 1, r.m);
@@ -778,7 +778,7 @@ class Engine : public EngineBase {
   // level by level: constraints through witness_level_body (assign or check), directives through solver_body.
   struct ProgDev {
     ProgData d;
-    DevBuf<uint32_t> kind, arg, in_ptr, out_ptr, out_cols, lc_ptr, lc_col, rows, out_var, dirs;
+    DevBuf<uint32_t> kind, arg, in_ptr, out_ptr, out_cols, lc_ptr, lc_col, rows, out_var, dirs, arg_cols;
     DevBuf<Fr> lc_val;
     std::vector<uint64_t> z_host;   // the assignment of the last compute_witness / set_witness (m x 4 words), for public_inputs
     uint64_t fp[2] = {0, 0};        // content fingerprint of the program file
@@ -829,7 +829,7 @@ class Engine : public EngineBase {
     try {
       upload(p->kind, d.d_kind); upload(p->arg, d.d_arg); upload(p->in_ptr, d.d_in_ptr); upload(p->out_ptr, d.d_out_ptr);
       upload(p->out_cols, d.d_out_cols); upload(p->lc_ptr, d.lc_ptr); upload(p->lc_col, d.lc_col);
-      upload(p->rows, d.rows); upload(p->out_var, d.out_var); upload(p->dirs, d.dirs);
+      upload(p->rows, d.rows); upload(p->out_var, d.out_var); upload(p->dirs, d.dirs); upload(p->arg_cols, d.arg_cols);
       const size_t nt = d.lc_col.size();
       p->lc_val.alloc(nt ? nt : 1);
       h2d(st_, p->lc_val.p, d.lc_val.data(), nt * FRB);
@@ -874,6 +874,47 @@ class Engine : public EngineBase {
     }
   }
 
+  // the refusals of a witness call, before any launch: input count, canonical inputs (K sets of n_inputs), schedulable
+  // program, no solver without a device path
+  void prog_check_inputs(const ProgData& d, const uint64_t* inputs, uint64_t n_inputs, uint64_t K) {
+    if (n_inputs != d.arg_ids.size())
+      throw Error(ZKB_E_ARG, "WrongInputCount: expected " + std::to_string(d.arg_ids.size()) + ", received " + std::to_string(n_inputs));
+    if (!d.schedule_error.empty()) throw Error(ZKB_E_FORMAT, "program cannot be executed: " + d.schedule_error);
+    if (d.n_unsupported) throw Error(ZKB_E_ARG, "the program calls a solver that has no device path (Zir function / embed gadget)");
+    uint32_t mod[8];
+    fr_modulus(mod);
+    for (uint64_t i = 0; i < K * n_inputs; i++)
+      if (!prog_detail::canonical((const uint8_t*)(inputs + 4 * i), mod))
+        throw Error(ZKB_E_ARG, "input is not a canonical field element" + (K > 1 ? " (input set " + std::to_string(i / n_inputs) + ")" : std::string()));
+  }
+  static size_t witness_file_len(const ProgData& d) {   // all witness files of one program have this length
+    return 8 + 40 * (size_t)std::count(d.defined.begin(), d.defined.end(), (uint8_t)1);
+  }
+
+  // The level sweep of K input sets: constraints through witness_level_body, directives through solver_body, one launch each
+  // per level whatever K is.  zp: interleaved Montgomery assignments z[col * K + k] (m_ext columns), inputs in place;
+  // flag[k] (0xFFFFFFFF on entry) receives set k's first violated row.
+  void prog_levels(const ProgDev& p, R1cs& r, uint32_t K, Fr* zp, uint32_t* flag, uint32_t flags) {
+    const ProgData& d = p.d;
+    const uint32_t* rpA = r.rowptr[0].p; const uint32_t* clA = r.col[0].p; const Fr* vlA = r.val[0].p;
+    const uint32_t* rpB = r.rowptr[1].p; const uint32_t* clB = r.col[1].p; const Fr* vlB = r.val[1].p;
+    const uint32_t* rpC = r.rowptr[2].p; const uint32_t* clC = r.col[2].p; const Fr* vlC = r.val[2].p;
+    const uint32_t* pr = p.rows.p; const uint32_t* po = p.out_var.p; const uint32_t* pd = p.dirs.p;
+    const uint32_t* kd = p.kind.p; const uint32_t* ar = p.arg.p; const uint32_t* ip = p.in_ptr.p; const uint32_t* op = p.out_ptr.p;
+    const uint32_t* oc = p.out_cols.p; const uint32_t* lp = p.lc_ptr.p; const uint32_t* lc = p.lc_col.p; const Fr* lv = p.lc_val.p;
+    for (uint32_t l = 1; l <= d.n_levels; l++) {
+      const uint32_t rlo = d.row_level_ptr[l - 1], rhi = d.row_level_ptr[l], dlo = d.dir_level_ptr[l - 1], dhi = d.dir_level_ptr[l];
+      if (rhi > rlo)
+        launch<k_witness_level>(st_, (size_t)(rhi - rlo) * K, ZKB_LAMBDA(size_t t) {
+          witness_level_body<Fr>(rpA, clA, vlA, rpB, clB, vlB, rpC, clC, vlC, zp, pr, po, rlo, rhi, K, flag, (uint32_t)t);
+        });
+      if (dhi > dlo)
+        launch<k_solver_level, 64>(st_, (size_t)(dhi - dlo) * K, ZKB_LAMBDA(size_t t) {
+          solver_body<Fr>(kd, ar, ip, op, oc, lp, lc, lv, zp, pd, dlo, dhi, K, flags, (uint32_t)t);
+        });
+    }
+  }
+
   // inputs: one canonical field element per program argument.  Returns the first unsatisfied constraint or ~0; on success
   // the assignment stays resident in the program's R1CS (zkb_groth16_prove_resident can follow) and `wit_out` receives the
   // witness FILE bytes (ir/witness.rs:44-53) when it is non-null.
@@ -881,14 +922,7 @@ class Engine : public EngineBase {
                                 size_t* wit_len) override {
     ProgDev& p = get_prog(h);
     const ProgData& d = p.d;
-    if (n_inputs != d.arg_ids.size())
-      throw Error(ZKB_E_ARG, "WrongInputCount: expected " + std::to_string(d.arg_ids.size()) + ", received " + std::to_string(n_inputs));
-    if (!d.schedule_error.empty()) throw Error(ZKB_E_FORMAT, "program cannot be executed: " + d.schedule_error);
-    if (d.n_unsupported) throw Error(ZKB_E_ARG, "the program calls a solver that has no device path (Zir function / embed gadget)");
-    uint32_t mod[8];
-    fr_modulus(mod);
-    for (uint64_t i = 0; i < n_inputs; i++)
-      if (!prog_detail::canonical((const uint8_t*)(inputs + 4 * i), mod)) throw Error(ZKB_E_ARG, "input is not a canonical field element");
+    prog_check_inputs(d, inputs, n_inputs, 1);
     R1cs& r = get_r1cs(d.r1cs);
     std::vector<uint64_t> z((size_t)d.m_ext * 4, 0);
     z[0] = 1;
@@ -900,25 +934,7 @@ class Engine : public EngineBase {
     dev_fill_ff(st_, d_flag.p, 4);
     tm.begin("witness_eval");
     convert(zc.p, zm.p, 0, d.m_ext);
-    const uint32_t* rpA = r.rowptr[0].p; const uint32_t* clA = r.col[0].p; const Fr* vlA = r.val[0].p;
-    const uint32_t* rpB = r.rowptr[1].p; const uint32_t* clB = r.col[1].p; const Fr* vlB = r.val[1].p;
-    const uint32_t* rpC = r.rowptr[2].p; const uint32_t* clC = r.col[2].p; const Fr* vlC = r.val[2].p;
-    Fr* zp = zm.p;
-    uint32_t* flag = d_flag.p;
-    const uint32_t* pr = p.rows.p; const uint32_t* po = p.out_var.p; const uint32_t* pd = p.dirs.p;
-    const uint32_t* kd = p.kind.p; const uint32_t* ar = p.arg.p; const uint32_t* ip = p.in_ptr.p; const uint32_t* op = p.out_ptr.p;
-    const uint32_t* oc = p.out_cols.p; const uint32_t* lp = p.lc_ptr.p; const uint32_t* lc = p.lc_col.p; const Fr* lv = p.lc_val.p;
-    for (uint32_t l = 1; l <= d.n_levels; l++) {
-      const uint32_t rlo = d.row_level_ptr[l - 1], rhi = d.row_level_ptr[l], dlo = d.dir_level_ptr[l - 1], dhi = d.dir_level_ptr[l];
-      if (rhi > rlo)
-        launch<k_witness_level>(st_, rhi - rlo, ZKB_LAMBDA(size_t t) {
-          witness_level_body<Fr>(rpA, clA, vlA, rpB, clB, vlB, rpC, clC, vlC, zp, pr, po, rlo, rhi, flag, (uint32_t)t);
-        });
-      if (dhi > dlo)
-        launch<k_solver_level, 64>(st_, dhi - dlo, ZKB_LAMBDA(size_t t) {
-          solver_body<Fr>(kd, ar, ip, op, oc, lp, lc, lv, zp, pd, dlo, dhi, flags, (uint32_t)t);
-        });
-    }
+    prog_levels(p, r, 1, zm.p, d_flag.p, flags);
     convert(zm.p, zc.p, 1, d.m_ext);
     tm.end();
     uint32_t first = 0;
@@ -931,7 +947,7 @@ class Engine : public EngineBase {
     r.has_z = true;
     r.sparse_z = assignment_is_sparse(z.data(), d.m);
     p.z_host.assign(z.begin(), z.begin() + (size_t)d.m * 4);
-    if (wit_len) *wit_len = 8 + 40 * (size_t)std::count(d.defined.begin(), d.defined.end(), (uint8_t)1);
+    if (wit_len) *wit_len = witness_file_len(d);
     if (wit_out) {
       std::vector<uint8_t> bytes;
       witness_write(d, z.data(), bytes);
@@ -940,6 +956,95 @@ class Engine : public EngineBase {
     }
     return ~0ull;
   }
+
+  // ---- batches of input sets (zkb_prog_compute_witness_batch / zkb_prog_prove_batch)
+  // The level schedule, the matrices and the directive tables do not depend on the inputs, so one sweep serves K input sets
+  // with every launch K times wider; the assignments come out in the interleaved Montgomery layout the batched SpMV reads.
+  // Neither batch call touches the program's resident assignment (z_host, the R1CS's z_canon).
+
+  // most input sets one sweep holds: the 32-bit thread index of its launches (statements x K, columns x K)
+  static uint64_t prog_sweep_max(const ProgData& d) {
+    const uint64_t widest = std::max<uint64_t>({(uint64_t)d.m_ext, (uint64_t)d.rows.size(), (uint64_t)d.dirs.size(), (uint64_t)d.arg_ids.size() + 1});
+    return ((1ull << 32) - 1) / widest;
+  }
+  // upload K input sets and scatter them into zm = interleaved Montgomery z (m_ext x K, `one` in column 0, every other column
+  // zero), then sweep the levels; flag[k] receives set k's first violated row
+  void prog_sweep_batch(const ProgDev& p, uint32_t K, const uint64_t* inputs, uint32_t flags, Fr* zm, uint32_t* flag) {
+    const ProgData& d = p.d;
+    R1cs& r = get_r1cs(d.r1cs);
+    const uint32_t n_in = (uint32_t)d.arg_ids.size();
+    DevBuf<Fr> din((size_t)K * n_in);
+    h2d(st_, din.p, inputs, (size_t)K * n_in * FRB);
+    dev_zero(st_, zm, (size_t)K * d.m_ext * FRB);
+    dev_fill_ff(st_, flag, (size_t)K * 4);
+    const Fr* in = din.p;
+    const uint32_t* ac = p.arg_cols.p;
+    launch<k_fr_convert>(st_, (size_t)K * (n_in + 1), ZKB_LAMBDA(size_t t) {
+      const uint32_t k = (uint32_t)(t % K), i = (uint32_t)(t / K);
+      if (i == 0) zm[k] = Fr::one();
+      else zm[(size_t)ac[i - 1] * K + k] = Fr::to_mont(in[(size_t)k * n_in + i - 1]);
+    });
+    prog_levels(p, r, K, zm, flag, flags);
+  }
+  // one pass of K input sets to the host: z_out gets K canonical assignments of m_ext columns back to back, first[k] set k's
+  // first violated row or ~0
+  void prog_witness_pass(const ProgDev& p, uint32_t K, const uint64_t* inputs, uint32_t flags, uint64_t* z_out, uint64_t* first) {
+    const size_t me = p.d.m_ext;
+    DevBuf<Fr> zm(K * me), zc(K * me);
+    DevBuf<uint32_t> d_flag(K);
+    prog_sweep_batch(p, K, inputs, flags, zm.p, d_flag.p);
+    const Fr* zi = zm.p; Fr* zo = zc.p;
+    launch<k_fr_convert>(st_, K * me, ZKB_LAMBDA(size_t t) { zo[t] = Fr::from_mont(zi[(t % me) * K + t / me]); });
+    std::vector<uint32_t> f(K);
+    d2h(st_, f.data(), d_flag.p, (size_t)K * 4);
+    d2h(st_, z_out, zc.p, K * me * FRB);
+    stream_sync(st_);
+    for (uint32_t k = 0; k < K; k++) first[k] = f[k] == 0xFFFFFFFFu ? ~0ull : (uint64_t)f[k];
+  }
+  // input sets per witness pass: the sweep's thread index, ZKB_OPT_BATCH_PASS_MAX, and free HBM (two m_ext x K vectors)
+  uint32_t prog_witness_pass_size(const ProgData& d, uint32_t K) {
+    uint64_t kmax = std::min<uint64_t>(K, prog_sweep_max(d));
+    if (opts.batch_pass_max > 0) kmax = std::min<uint64_t>(kmax, (uint64_t)opts.batch_pass_max);
+#if !defined(ZKB_EMU)
+    size_t free_b = 0, total_b = 0;
+    ZKB_CUDA(cudaMemGetInfo(&free_b, &total_b));
+    const size_t reserve = (size_t)1 << 30, per = (2 * (size_t)d.m_ext + d.arg_ids.size()) * FRB + 4;
+    const uint64_t fit = free_b > reserve ? (free_b - reserve) / per : 0;
+    kmax = std::min<uint64_t>(kmax, fit);
+#endif
+    if (kmax == 0) throw Error(ZKB_E_OOM, "not even one input set fits in device memory");
+    return (uint32_t)kmax;
+  }
+  // K input sets (K x n_inputs canonical elements) -> K witness files of one length back to back in wit_out; first[k] set k's
+  // first violated row (its file zero-filled) or ~0.  Returns whether every set was satisfied.
+  bool prog_compute_witness_batch(uint64_t h, uint32_t K, const uint64_t* inputs, uint64_t n_inputs, uint32_t flags, uint8_t* wit_out,
+                                  size_t cap, size_t* wit_len, uint64_t* first) override {
+    if (K == 0) throw Error(ZKB_E_ARG, "empty batch");
+    ProgDev& p = get_prog(h);
+    const ProgData& d = p.d;
+    prog_check_inputs(d, inputs, n_inputs, K);
+    const size_t len = witness_file_len(d);
+    if (wit_out && cap < K * len) throw Error(ZKB_E_ARG, "witness buffer too small");
+    if (wit_len) *wit_len = len;
+    const uint32_t kp = prog_witness_pass_size(d, K);
+    std::vector<uint64_t> z((size_t)kp * d.m_ext * 4);
+    bool all = true;
+    for (uint32_t k0 = 0; k0 < K; k0 += kp) {
+      const uint32_t cnt = std::min(kp, K - k0);
+      prog_witness_pass(p, cnt, inputs + (size_t)k0 * n_inputs * 4, flags, z.data(), first + k0);
+      for (uint32_t k = 0; k < cnt; k++) all &= first[k0 + k] == ~0ull;
+      if (!wit_out) continue;
+      host_parallel(cnt, [&](uint32_t k) {
+        uint8_t* dst = wit_out + (size_t)(k0 + k) * len;
+        if (first[k0 + k] != ~0ull) { memset(dst, 0, len); return; }
+        std::vector<uint8_t> bytes;
+        witness_write(d, z.data() + (size_t)k * d.m_ext * 4, bytes);
+        memcpy(dst, bytes.data(), len);
+      });
+    }
+    return all;
+  }
+
   // witness file -> resident assignment of the program's R1CS (what `generate-proof -w witness` reads, generate_proof.rs:161-166)
   void prog_set_witness(uint64_t h, const uint8_t* wit, size_t len) override {
     ProgDev& p = get_prog(h);
@@ -955,11 +1060,8 @@ class Engine : public EngineBase {
     if (cap_elems < p.d.m) throw Error(ZKB_E_ARG, "assignment buffer too small");
     memcpy(z_out, p.z_host.data(), p.z_host.size() * 8);
   }
-  // public arguments in declaration order, then the return values ~out_0.. (ir/mod.rs:278-288), from the current assignment
-  uint64_t prog_public_inputs(uint64_t h, uint64_t* out, uint64_t cap) override {
-    ProgDev& p = get_prog(h);
-    const ProgData& d = p.d;
-    if (p.z_host.size() != (size_t)d.m * 4) throw Error(ZKB_E_ARG, "the program has no assignment yet");
+  // the columns of the public inputs: public arguments in declaration order, then the return values ~out_0.. (ir/mod.rs:278-288)
+  static std::vector<uint32_t> public_cols(const ProgData& d) {
     std::vector<uint32_t> cols;
     for (size_t i = 0; i < d.arg_ids.size(); i++) if (!d.arg_private[i]) cols.push_back(d.arg_cols[i]);
     for (uint32_t k = 0; k < d.n_ret; k++) {
@@ -969,6 +1071,13 @@ class Engine : public EngineBase {
       if (c == d.ni) throw Error(ZKB_E_FORMAT, "return value ~out_" + std::to_string(k) + " does not occur in the constraints");
       cols.push_back(c);
     }
+    return cols;
+  }
+  // public arguments in declaration order, then the return values ~out_0.. (ir/mod.rs:278-288), from the current assignment
+  uint64_t prog_public_inputs(uint64_t h, uint64_t* out, uint64_t cap) override {
+    ProgDev& p = get_prog(h);
+    if (p.z_host.size() != (size_t)p.d.m * 4) throw Error(ZKB_E_ARG, "the program has no assignment yet");
+    const std::vector<uint32_t> cols = public_cols(p.d);
     if (out) {
       if (cols.size() > cap) throw Error(ZKB_E_ARG, "public input buffer too small");
       for (size_t i = 0; i < cols.size(); i++) memcpy(out + 4 * i, &p.z_host[4 * (size_t)cols[i]], 32);
@@ -2036,10 +2145,10 @@ class Engine : public EngineBase {
   static constexpr uint32_t BATCH_SLOTS_MIN_LOG = 18;
   static constexpr int SPMV_GROUP = 4;   // assignments per thread of the batched SpMV
 
-  // device bytes of one pass of K proofs (the buffers BatchState grows to), an upper estimate
-  size_t batch_bytes(const Pk& pk, const R1cs& rc, uint64_t K, uint32_t pre_c_z) const {
+  // device bytes of one pass of K proofs (the buffers BatchState grows to, plus `extra` per proof), an upper estimate
+  size_t batch_bytes(const Pk& pk, const R1cs& rc, uint64_t K, uint32_t pre_c_z, size_t extra) const {
     const uint64_t n = 1ull << rc.log_n;
-    size_t bytes = (size_t)K * (2 * rc.m + 4 * n) * FRB;
+    size_t bytes = (size_t)K * ((2 * rc.m + 4 * n) * FRB + extra);
     auto plan = [&](uint64_t cnt, uint32_t nviews, uint32_t pre_c, std::initializer_list<size_t> xs) -> size_t {
       if (!cnt) return 0;
       const uint32_t c = plan_c(cnt, pre_c), W = plan_w(c);
@@ -2056,7 +2165,7 @@ class Engine : public EngineBase {
     return bytes;
   }
   // proofs per pass: the uint32 bound of the sorted lists, ZKB_OPT_BATCH_PASS_MAX, and what fits in free HBM
-  uint32_t batch_pass_size(const Pk& pk, const R1cs& rc, uint32_t K, uint32_t pre_c_z) {
+  uint32_t batch_pass_size(const Pk& pk, const R1cs& rc, uint32_t K, uint32_t pre_c_z, size_t extra = 0) {
     uint64_t kmax = std::min<uint64_t>(plan_max_batch(pk.hi - pk.lo, 3, pre_c_z), plan_max_batch(pk.hhi - pk.hlo, 1, pk.pre_ch));
     if (opts.batch_pass_max > 0) kmax = std::min<uint64_t>(kmax, (uint64_t)opts.batch_pass_max);
     kmax = std::min<uint64_t>(kmax, K);
@@ -2066,7 +2175,7 @@ class Engine : public EngineBase {
     ZKB_CUDA(cudaMemGetInfo(&free_b, &total_b));
     const size_t reserve = (size_t)1 << 30, have = free_b + batch_.device_bytes();
     const size_t avail = have > reserve ? have - reserve : 0;
-    for (size_t need = batch_bytes(pk, rc, kmax, pre_c_z); kmax > 1 && need > avail; need = batch_bytes(pk, rc, kmax, pre_c_z))
+    for (size_t need = batch_bytes(pk, rc, kmax, pre_c_z, extra); kmax > 1 && need > avail; need = batch_bytes(pk, rc, kmax, pre_c_z, extra))
       kmax = std::max<uint64_t>(1, std::min<uint64_t>(kmax - 1, (uint64_t)((double)kmax * avail / need)));
 #endif
     return (uint32_t)kmax;
@@ -2082,16 +2191,22 @@ class Engine : public EngineBase {
     for (auto& f : fs) f.get();
   }
 
-  void prove_batch(uint64_t pkh, uint64_t rh, uint32_t K, const uint64_t* z, const uint64_t* r, const uint64_t* s,
-                   uint8_t* proofs_out) override {
+  // the refusals of a batch of proofs, before any launch
+  void batch_check(uint32_t K, const Pk& pk, const R1cs& rc) {
     if (K == 0) throw Error(ZKB_E_ARG, "empty batch");
-    Pk& pk = get_pk(pkh);
-    R1cs& rc = get_r1cs(rh);
     if (pk.m != rc.m || pk.ni != rc.ni) throw Error(ZKB_E_ARG, "proving key does not match the R1CS (variable counts)");
     if (pk.hl + 1 != ((uint64_t)1 << rc.log_n)) throw Error(ZKB_E_ARG, "proving key does not match the R1CS (domain size)");
     if (pk.world != 1) throw Error(ZKB_E_ARG, "a batch needs a key loaded whole (world = 1)");
     for (auto& sl : slots_)
       if (sl.state != 0) throw Error(ZKB_E_ARG, "a proof is in flight on this context (collect it first)");
+  }
+
+  void prove_batch(uint64_t pkh, uint64_t rh, uint32_t K, const uint64_t* z, const uint64_t* r, const uint64_t* s,
+                   uint8_t* proofs_out) override {
+    if (K == 0) throw Error(ZKB_E_ARG, "empty batch");
+    Pk& pk = get_pk(pkh);
+    R1cs& rc = get_r1cs(rh);
+    batch_check(K, pk, rc);
     const size_t zw = (size_t)rc.m * 4, pb = 8 * FQB;    // words per assignment, bytes per proof
     if (rc.log_n >= BATCH_SLOTS_MIN_LOG || K == 1) {     // large circuits and single proofs: the two-slot pipeline
       uint64_t prev = 0;
@@ -2124,6 +2239,8 @@ class Engine : public EngineBase {
     timings = all;
   }
 
+  // z == nullptr: the pass's assignments are already in batch_.zc (canonical, back to back) and batch_.zm (Montgomery,
+  // interleaved with stride K), written by prog_prove_batch's witness sweep
   void batch_pass(const Pk& pk, R1cs& rc, uint32_t K, const uint64_t* z, const uint64_t* r, const uint64_t* s, uint32_t pre_c_z,
                   uint8_t* proofs_out, std::vector<std::pair<const char*, double>>& times) {
     BatchState& b = batch_;
@@ -2137,13 +2254,15 @@ class Engine : public EngineBase {
     });
     b.zc.ensure(K * m); b.zm.ensure(K * m); b.v.ensure(3 * K * n); b.h.ensure(K * n);
     StageTimer tm(st_);
-    tm.begin("h2d_z_batch");
-    h2d(st_, b.zc.p, z, K * m * FRB);
-    tm.end();
+    if (z) {
+      tm.begin("h2d_z_batch");
+      h2d(st_, b.zc.p, z, K * m * FRB);
+      tm.end();
+    }
     tm.begin("witness_map_batch");
     {
       const Fr* zc = b.zc.p; Fr* zm = b.zm.p;
-      launch<k_fr_convert>(st_, K * m, ZKB_LAMBDA(size_t t) { zm[(t % m) * K + t / m] = Fr::to_mont(zc[t]); });
+      if (z) launch<k_fr_convert>(st_, K * m, ZKB_LAMBDA(size_t t) { zm[(t % m) * K + t / m] = Fr::to_mont(zc[t]); });
       const uint32_t* rpA = rc.rowptr[0].p; const uint32_t* clA = rc.col[0].p; const Fr* vlA = rc.val[0].p;
       const uint32_t* rpB = rc.rowptr[1].p; const uint32_t* clB = rc.col[1].p; const Fr* vlB = rc.val[1].p;
       const uint32_t* rpC = rc.rowptr[2].p; const uint32_t* clC = rc.col[2].p; const Fr* vlC = rc.val[2].p;
@@ -2200,6 +2319,107 @@ class Engine : public EngineBase {
                     proofs_out + (size_t)k * 8 * FQB);
     });
     times.push_back({"host_tails_batch", std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count()});
+  }
+
+  // Inputs -> K proofs of one program under one key, the assignments resident on the device between witness generation
+  // and proving.  Below BATCH_SLOTS_MIN_LOG (K > 1) the witness sweep of a pass writes straight into the batch buffers:
+  // columns [0, m) of its interleaved z are batch_.zm's layout (directive-only columns sit at m .. m_ext), one kernel fills
+  // the canonical batch_.zc and the public columns, and batch_pass proves from there.  Otherwise the witnesses go to the host
+  // and prove_batch drives the two-slot pipeline.  public_out: K x (public inputs) elements; a set whose witness fails gets
+  // first[k] = its first violated row and zero-filled proof and public slots.  Returns whether every set was satisfied.
+  bool prog_prove_batch(uint64_t ph, uint64_t pkh, uint32_t K, const uint64_t* inputs, uint64_t n_inputs, uint32_t flags,
+                        const uint64_t* r, const uint64_t* s, uint8_t* proofs_out, uint64_t* public_out, uint64_t public_cap,
+                        uint64_t* first) override {
+    if (K == 0) throw Error(ZKB_E_ARG, "empty batch");
+    ProgDev& p = get_prog(ph);
+    const ProgData& d = p.d;
+    Pk& pk = get_pk(pkh);
+    R1cs& rc = get_r1cs(d.r1cs);
+    batch_check(K, pk, rc);
+    prog_check_inputs(d, inputs, n_inputs, K);
+    const std::vector<uint32_t> pub = public_cols(d);
+    const size_t np = pub.size(), pb = 8 * FQB, me = d.m_ext, m = d.m, ni = d.ni;
+    if (public_out && public_cap < K * np) throw Error(ZKB_E_ARG, "public input buffer too small");
+    auto finish = [&](uint32_t k, const uint64_t* zk) {   // set k's public inputs from its assignment, or zeroed slots
+      if (first[k] != ~0ull) {
+        memset(proofs_out + (size_t)k * pb, 0, pb);
+        if (public_out) memset(public_out + (size_t)k * np * 4, 0, np * FRB);
+      } else if (public_out) {
+        for (size_t i = 0; i < np; i++) memcpy(public_out + ((size_t)k * np + i) * 4, zk + 4 * (size_t)pub[i], 32);
+      }
+    };
+    if (rc.log_n >= BATCH_SLOTS_MIN_LOG || K == 1) {
+      std::vector<uint64_t> zall((size_t)K * m * 4);
+      const uint32_t kw = prog_witness_pass_size(d, K);
+      std::vector<uint64_t> z((size_t)kw * me * 4);
+      for (uint32_t k0 = 0; k0 < K; k0 += kw) {
+        const uint32_t cnt = std::min(kw, K - k0);
+        prog_witness_pass(p, cnt, inputs + (size_t)k0 * n_inputs * 4, flags, z.data(), first + k0);
+        for (uint32_t k = 0; k < cnt; k++) memcpy(&zall[(size_t)(k0 + k) * m * 4], &z[(size_t)k * me * 4], m * FRB);
+      }
+      prove_batch(pkh, d.r1cs, K, zall.data(), r, s, proofs_out);
+      bool all = true;
+      for (uint32_t k = 0; k < K; k++) { finish(k, &zall[(size_t)k * m * 4]); all &= first[k] == ~0ull; }
+      return all;
+    }
+    // pass size: what fits in either z-MSM mode, with the wider interleaved z, the inputs and the public columns per proof
+    const size_t extra = (me - m + n_inputs + ni) * FRB + 4;
+    uint32_t kp = std::min(batch_pass_size(pk, rc, K, pk.pre_cz, extra), batch_pass_size(pk, rc, K, 0, extra));
+    kp = (uint32_t)std::min<uint64_t>(kp, prog_sweep_max(d));
+    // one z-MSM mode for the whole batch, from the assignments prove_batch would sample.  Several passes: the sampled sets
+    // are swept first; one pass: they are read back from its sweep.
+    const uint32_t ns = std::min(K, 8u);
+    std::vector<uint32_t> sample(ns);
+    for (uint32_t i = 0; i < ns; i++) sample[i] = (uint32_t)((size_t)i * K / ns);
+    int pre_c_z = -1;
+    if (kp < K) {
+      std::vector<uint64_t> sin((size_t)ns * n_inputs * 4), sz((size_t)ns * me * 4), sf(ns);
+      for (uint32_t i = 0; i < ns; i++) memcpy(&sin[(size_t)i * n_inputs * 4], inputs + (size_t)sample[i] * n_inputs * 4, n_inputs * FRB);
+      prog_witness_pass(p, ns, sin.data(), flags, sz.data(), sf.data());
+      uint32_t sparse = 0;
+      for (uint32_t i = 0; i < ns; i++) sparse += assignment_is_sparse(&sz[(size_t)i * me * 4], m);
+      pre_c_z = z_window_mode(2 * sparse > ns) ? 0 : (int)pk.pre_cz;
+      kp = batch_pass_size(pk, rc, K, (uint32_t)pre_c_z, extra);
+      kp = (uint32_t)std::min<uint64_t>(kp, prog_sweep_max(d));
+    }
+    BatchState& b = batch_;
+    std::vector<std::pair<const char*, double>> all_t, part;
+    std::vector<uint64_t> hpub, zs(m * 4);
+    std::vector<uint32_t> f;
+    bool all = true;
+    for (uint32_t k0 = 0; k0 < K; k0 += kp) {
+      const uint32_t cnt = std::min(kp, K - k0);
+      b.zc.ensure((size_t)cnt * m); b.zm.ensure((size_t)cnt * me);
+      DevBuf<uint32_t> d_flag(cnt);
+      DevBuf<Fr> d_pub((size_t)cnt * ni);
+      prog_sweep_batch(p, cnt, inputs + (size_t)k0 * n_inputs * 4, flags, b.zm.p, d_flag.p);
+      const Fr* zi = b.zm.p; Fr* zo = b.zc.p; Fr* po = d_pub.p;
+      launch<k_fr_convert>(st_, (size_t)cnt * m, ZKB_LAMBDA(size_t t) {
+        const size_t k = t / m, col = t % m;
+        const Fr v = Fr::from_mont(zi[col * cnt + k]);
+        zo[t] = v;
+        if (col < ni) po[k * ni + col] = v;
+      });
+      f.resize(cnt); hpub.resize((size_t)cnt * ni * 4);
+      d2h(st_, f.data(), d_flag.p, (size_t)cnt * 4);
+      d2h(st_, hpub.data(), d_pub.p, (size_t)cnt * ni * FRB);
+      stream_sync(st_);
+      for (uint32_t k = 0; k < cnt; k++) first[k0 + k] = f[k] == 0xFFFFFFFFu ? ~0ull : (uint64_t)f[k];
+      if (pre_c_z < 0) {   // the whole batch is this pass
+        uint32_t sparse = 0;
+        for (uint32_t i = 0; i < ns; i++) {
+          d2h(st_, zs.data(), b.zc.p + (size_t)sample[i] * m, m * FRB);
+          stream_sync(st_);
+          sparse += assignment_is_sparse(zs.data(), m);
+        }
+        pre_c_z = z_window_mode(2 * sparse > ns) ? 0 : (int)pk.pre_cz;
+      }
+      batch_pass(pk, rc, cnt, nullptr, r + 4 * (size_t)k0, s + 4 * (size_t)k0, (uint32_t)pre_c_z, proofs_out + k0 * pb, part);
+      all_t.insert(all_t.end(), part.begin(), part.end());
+      for (uint32_t k = 0; k < cnt; k++) { finish(k0 + k, &hpub[(size_t)k * ni * 4]); all &= first[k0 + k] == ~0ull; }
+    }
+    timings = all_t;
+    return all;
   }
 
   // ------------------------------------------------------------------------------ standalone MSM (tests / microbench)

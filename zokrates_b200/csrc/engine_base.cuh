@@ -25,7 +25,7 @@ struct Options {
   int64_t ntt_kernel = 2;     // ZKB_OPT_NTT_KERNEL: 2 = four-step twiddles / cp.async tile load (ntt_tile.cuh), 1 = the round-1 tile pass
   int64_t pk_cache = 1;       // ZKB_OPT_PK_CACHE: share proving keys by content and keep the last released one resident
   int64_t bitsum_radix = 2;   // ZKB_OPT_BITSUM_RADIX: bucket-reduction levels of radix 2 (1 dependent addition per launch) or 8 (7)
-  int64_t batch_pass_max = 0; // ZKB_OPT_BATCH_PASS_MAX: most proofs of zkb_groth16_prove_batch per pass; 0 = as many as fit in HBM
+  int64_t batch_pass_max = 0; // ZKB_OPT_BATCH_PASS_MAX: most proofs or input sets of one batch pass; 0 = as many as fit in HBM
 };
 
 struct EngineBase {
@@ -69,6 +69,11 @@ struct EngineBase {
   virtual void prog_free(uint64_t h) = 0;
   virtual uint64_t prog_compute_witness(uint64_t h, const uint64_t* inputs, uint64_t n_inputs, uint32_t flags, uint8_t* wit_out,
                                         size_t cap, size_t* wit_len) = 0;
+  virtual bool prog_compute_witness_batch(uint64_t h, uint32_t count, const uint64_t* inputs, uint64_t n_inputs, uint32_t flags,
+                                          uint8_t* wit_out, size_t cap, size_t* wit_len, uint64_t* first_unsat) = 0;
+  virtual bool prog_prove_batch(uint64_t h, uint64_t pk, uint32_t count, const uint64_t* inputs, uint64_t n_inputs, uint32_t flags,
+                                const uint64_t* r, const uint64_t* s, uint8_t* proofs_out, uint64_t* public_out, uint64_t public_cap,
+                                uint64_t* first_unsat) = 0;
   virtual void prog_set_witness(uint64_t h, const uint8_t* wit, size_t len) = 0;
   virtual uint64_t prog_public_inputs(uint64_t h, uint64_t* out, uint64_t cap) = 0;
   virtual void prog_assignment(uint64_t h, uint64_t* z_out, uint64_t cap_elems) = 0;

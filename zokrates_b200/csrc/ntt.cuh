@@ -301,7 +301,10 @@ ZKB_HDN inline void spmv_batch_body(const uint32_t* rowptr, const uint32_t* col,
 // ---- levelised witness evaluation / R1CS satisfaction check ------------------------------------------------
 // Restates the per-statement rule of zokrates_interpreter/src/lib.rs:61-138 on the R1CS rows: a constraint whose linear side
 // is one fresh variable with coefficient one ASSIGNS it the value of the quadratic side, every other constraint is CHECKED
-// (`Error::UnsatisfiedConstraint`).  The statements of one dependency level are independent: one thread each.
+// (`Error::UnsatisfiedConstraint`).  The statements of one dependency level are independent: one thread each per input set.
+// A batch of K input sets shares the schedule: z is INTERLEAVED, z[col * K + k] (the layout of spmv_batch_body), thread t
+// runs statement lo + t / K for set t % K, so the K threads of a statement read one CSR row and adjacent values; set k's
+// first violated row goes to first_unsat[k].  K = 1 is the single assignment.
 // rows == nullptr: row = index (check of the whole system); out_var == nullptr: every row is a check.
 static constexpr uint32_t WIT_CHECK = 0xFFFFFFFFu;
 #if defined(__CUDA_ARCH__)
@@ -310,25 +313,26 @@ __device__ __forceinline__ void zkb_atomic_min(uint32_t* p, uint32_t v) { atomic
 inline void zkb_atomic_min(uint32_t* p, uint32_t v) { if (v < *p) *p = v; }
 #endif
 template <class Fr>
-ZKB_HDN inline Fr csr_row_dot(const uint32_t* rowptr, const uint32_t* col, const Fr* val, const Fr* z, uint32_t row) {
+ZKB_HDN inline Fr csr_row_dot(const uint32_t* rowptr, const uint32_t* col, const Fr* val, const Fr* z, uint32_t K, uint32_t k,
+                              uint32_t row) {
   Fr acc = Fr::zero();
-  for (uint32_t k = rowptr[row]; k < rowptr[row + 1]; k++) acc = Fr::add(acc, Fr::mul(val[k], z[col[k]]));
+  for (uint32_t e = rowptr[row]; e < rowptr[row + 1]; e++) acc = Fr::add(acc, Fr::mul(val[e], z[(size_t)col[e] * K + k]));
   return acc;
 }
 template <class Fr>
 ZKB_HDN inline void witness_level_body(const uint32_t* rpA, const uint32_t* clA, const Fr* vlA, const uint32_t* rpB,
                                        const uint32_t* clB, const Fr* vlB, const uint32_t* rpC, const uint32_t* clC,
                                        const Fr* vlC, Fr* z, const uint32_t* rows, const uint32_t* out_var, uint32_t lo,
-                                       uint32_t hi, uint32_t* first_unsat, uint32_t t) {
-  const uint32_t i = lo + t;
+                                       uint32_t hi, uint32_t K, uint32_t* first_unsat, uint32_t t) {
+  const uint32_t i = lo + t / K, k = t % K;
   if (i >= hi) return;
   const uint32_t row = rows ? rows[i] : i;
-  const Fr q = Fr::mul(csr_row_dot<Fr>(rpA, clA, vlA, z, row), csr_row_dot<Fr>(rpB, clB, vlB, z, row));
+  const Fr q = Fr::mul(csr_row_dot<Fr>(rpA, clA, vlA, z, K, k, row), csr_row_dot<Fr>(rpB, clB, vlB, z, K, k, row));
   const uint32_t ov = out_var ? out_var[i] : WIT_CHECK;
   if (ov != WIT_CHECK) {
-    z[ov] = q;
-  } else if (!(q == csr_row_dot<Fr>(rpC, clC, vlC, z, row))) {
-    zkb_atomic_min(first_unsat, row);
+    z[(size_t)ov * K + k] = q;
+  } else if (!(q == csr_row_dot<Fr>(rpC, clC, vlC, z, K, k, row))) {
+    zkb_atomic_min(first_unsat + k, row);
   }
 }
 

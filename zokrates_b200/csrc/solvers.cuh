@@ -1,10 +1,12 @@
-// Solver directives on the device: one thread per directive of a dependency level.
+// Solver directives on the device: one thread per directive of a dependency level and input set.
 //
 // Restates `Interpreter::execute_solver` (/root/reference/zokrates_interpreter/src/lib.rs:249-307) and the out-of-range
 // `Bits` path (`try_solve_with_out_of_range_bits`, :140-165, taken when `should_try_out_of_range` is set and the width
 // covers the field, :94-101) for the simple solvers; `Zir` folded functions and the embed gadgets are front-end code and
 // have no device path (SOLVER_UNSUPPORTED).  Inputs are QuadCombs (left * right of two linear combinations, evaluated
 // like `evaluate_quad`, :366-378); outputs are written straight into the assignment vector (Montgomery form).
+// A batch of K input sets uses witness_level_body's layout (ntt.cuh): z[col * K + k], thread t runs directive lo + t / K for
+// set t % K; `flags` applies to the whole batch.
 #pragma once
 #include "fp.cuh"
 #include "prog.cuh"
@@ -12,9 +14,9 @@
 namespace zkb {
 
 template <class Fr>
-ZKB_HDN inline Fr lc_dot(const uint32_t* ptr, const uint32_t* col, const Fr* val, const Fr* z, uint32_t q) {
+ZKB_HDN inline Fr lc_dot(const uint32_t* ptr, const uint32_t* col, const Fr* val, const Fr* z, uint32_t K, uint32_t k, uint32_t q) {
   Fr acc = Fr::zero();
-  for (uint32_t k = ptr[q]; k < ptr[q + 1]; k++) acc = Fr::add(acc, Fr::mul(val[k], z[col[k]]));
+  for (uint32_t e = ptr[q]; e < ptr[q + 1]; e++) acc = Fr::add(acc, Fr::mul(val[e], z[(size_t)col[e] * K + k]));
   return acc;
 }
 
@@ -37,8 +39,8 @@ static constexpr uint32_t SOLVE_TRY_OUT_OF_RANGE = 1u;   // flags: Interpreter::
 template <class Fr>
 ZKB_HDN inline void solver_body(const uint32_t* kind, const uint32_t* arg, const uint32_t* in_ptr, const uint32_t* out_ptr,
                                 const uint32_t* out_cols, const uint32_t* lc_ptr, const uint32_t* lc_col, const Fr* lc_val, Fr* z,
-                                const uint32_t* dirs, uint32_t lo, uint32_t hi, uint32_t flags, uint32_t t) {
-  const uint32_t i = lo + t;
+                                const uint32_t* dirs, uint32_t lo, uint32_t hi, uint32_t K, uint32_t flags, uint32_t t) {
+  const uint32_t i = lo + t / K, kz = t % K;
   if (i >= hi) return;
   const uint32_t d = dirs[i];
   const uint32_t n_in = in_ptr[d + 1] - in_ptr[d];
@@ -46,7 +48,7 @@ ZKB_HDN inline void solver_body(const uint32_t* kind, const uint32_t* arg, const
   for (uint32_t j = 0; j < 3; j++) {
     if (j < n_in) {
       const uint32_t q = in_ptr[d] + j;
-      x[j] = Fr::mul(lc_dot<Fr>(lc_ptr, lc_col, lc_val, z, 2 * q), lc_dot<Fr>(lc_ptr, lc_col, lc_val, z, 2 * q + 1));
+      x[j] = Fr::mul(lc_dot<Fr>(lc_ptr, lc_col, lc_val, z, K, kz, 2 * q), lc_dot<Fr>(lc_ptr, lc_col, lc_val, z, K, kz, 2 * q + 1));
     } else {
       x[j] = Fr::zero();
     }
@@ -57,8 +59,8 @@ ZKB_HDN inline void solver_body(const uint32_t* kind, const uint32_t* arg, const
   switch (kind[d]) {
     case SOLVER_CONDITION_EQ: {          // x == 0 ? [0, 1] : [1, 1 / x]
       if (n_out < 2) return;
-      if (x[0].is_zero()) { z[oc[0]] = Fr::zero(); z[oc[1]] = one; }
-      else { z[oc[0]] = one; z[oc[1]] = Fr::inv(x[0]); }
+      if (x[0].is_zero()) { z[(size_t)oc[0] * K + kz] = Fr::zero(); z[(size_t)oc[1] * K + kz] = one; }
+      else { z[(size_t)oc[0] * K + kz] = one; z[(size_t)oc[1] * K + kz] = Fr::inv(x[0]); }
       return;
     }
     case SOLVER_BITS: {                  // big-endian bits, exactly `w` of them (the low w bits, zero-padded on the left)
@@ -78,28 +80,28 @@ ZKB_HDN inline void solver_body(const uint32_t* kind, const uint32_t* arg, const
       for (uint32_t k = 0; k < w && k < n_out; k++) {
         const uint32_t b = w - 1 - k;
         const uint32_t bit = b < 256 ? (v[b >> 5] >> (b & 31)) & 1u : 0u;
-        z[oc[k]] = bit ? one : Fr::zero();
+        z[(size_t)oc[k] * K + kz] = bit ? one : Fr::zero();
       }
       return;
     }
     case SOLVER_DIV:                     // x / y, 1 when y == 0 (checked_div(..).unwrap_or_else(T::one))
-      if (n_out) z[oc[0]] = x[1].is_zero() ? one : Fr::mul(x[0], Fr::inv(x[1]));
+      if (n_out) z[(size_t)oc[0] * K + kz] = x[1].is_zero() ? one : Fr::mul(x[0], Fr::inv(x[1]));
       return;
     case SOLVER_XOR:                     // x + y - 2 x y
-      if (n_out) { Fr xy = Fr::mul(x[0], x[1]); z[oc[0]] = Fr::sub(Fr::add(x[0], x[1]), Fr::dbl(xy)); }
+      if (n_out) { Fr xy = Fr::mul(x[0], x[1]); z[(size_t)oc[0] * K + kz] = Fr::sub(Fr::add(x[0], x[1]), Fr::dbl(xy)); }
       return;
     case SOLVER_OR:                      // x + y - x y
-      if (n_out) z[oc[0]] = Fr::sub(Fr::add(x[0], x[1]), Fr::mul(x[0], x[1]));
+      if (n_out) z[(size_t)oc[0] * K + kz] = Fr::sub(Fr::add(x[0], x[1]), Fr::mul(x[0], x[1]));
       return;
     case SOLVER_SHA_AXXA: {              // b c - (2 b c - b - c) a
       if (!n_out) return;
       Fr bc = Fr::mul(x[1], x[2]);
       Fr u = Fr::sub(Fr::sub(Fr::dbl(bc), x[1]), x[2]);
-      z[oc[0]] = Fr::sub(bc, Fr::mul(u, x[0]));
+      z[(size_t)oc[0] * K + kz] = Fr::sub(bc, Fr::mul(u, x[0]));
       return;
     }
     case SOLVER_SHA_CH:                  // a (b - c) + c
-      if (n_out) z[oc[0]] = Fr::add(Fr::mul(x[0], Fr::sub(x[1], x[2])), x[2]);
+      if (n_out) z[(size_t)oc[0] * K + kz] = Fr::add(Fr::mul(x[0], Fr::sub(x[1], x[2])), x[2]);
       return;
     case SOLVER_EUCLIDEAN_DIV: {         // integers: q = n / d (0 when d == 0), r = n - d q
       if (n_out < 2) return;
@@ -117,8 +119,8 @@ ZKB_HDN inline void solver_body(const uint32_t* kind, const uint32_t* arg, const
       }
       Fr qf, rf;
       for (int k = 0; k < 8; k++) { qf.v[k] = q[k]; rf.v[k] = rem[k]; }
-      z[oc[0]] = Fr::to_mont(qf);
-      z[oc[1]] = Fr::to_mont(rf);
+      z[(size_t)oc[0] * K + kz] = Fr::to_mont(qf);
+      z[(size_t)oc[1] * K + kz] = Fr::to_mont(rf);
       return;
     }
     default: return;                     // SOLVER_UNSUPPORTED: refused before the launch

@@ -291,3 +291,81 @@ def prove_from_inputs(prog: Prog, inputs: Sequence[int], proving_key, rng, devic
     by_var = dict(zip(r1cs.instance_vars[1:], public))
     ordered = [by_var[p.id] for p in prog.arguments if not p.private] + [by_var[Variable.public(i)] for i in range(prog.return_count)]
     return Proof.from_raw(c, raw, ordered)
+
+
+def _load_program(ctx, prog: Prog):
+    """zkb_prog_load of the program; refuses one whose solvers have no device path"""
+    from . import zir
+    h = ctx.prog_load(zir.write_prog(prog))
+    info = ctx.prog_info(h)
+    if info["unsupported_directives"]:
+        ctx.prog_free(h)
+        raise NotImplementedError("the program calls a solver that has no device path: use ir.Interpreter")
+    return h, info
+
+
+def _raise_first_failure(first):
+    for k, f in enumerate(first):
+        if f is not None:
+            raise UnsatisfiedConstraint(f"input set {k}: constraint {f} is not satisfied")
+
+
+def generate_witnesses(prog: Prog, inputs_list: Sequence[Sequence[int]], ctx=None, lib=None, try_out_of_range: bool = False) -> List[Witness]:
+    """`Interpreter::execute` of K input sets of one program in one level sweep on the device (zkb_prog_compute_witness_batch);
+    every program goes through the native front door.  Witness k equals `generate_witness(prog, inputs_list[k])`.  Raises
+    UnsatisfiedConstraint naming the first failing input set and its constraint, ValueError on a wrong input count."""
+    from . import backend
+    from ._lib import ZkbError
+    c = _curve(prog.curve)
+    for x in inputs_list:
+        if len(x) != len(prog.arguments):
+            raise ValueError(f"WrongInputCount: expected {len(prog.arguments)}, received {len(x)}")
+    if not inputs_list:
+        return []
+    ctx = ctx or backend.context(c, 0, lib)
+    with ctx.lock:
+        h, _ = _load_program(ctx, prog)
+        try:
+            try:
+                wits, first = ctx.prog_compute_witness_batch(h, [[int(v) % c.r for v in x] for x in inputs_list], try_out_of_range)
+            except ZkbError as e:
+                if e.code == 5:
+                    raise UnsatisfiedConstraint(str(e))
+                raise
+        finally:
+            ctx.prog_free(h)
+    _raise_first_failure(first)
+    return [Witness.read(w, c) for w in wits]
+
+
+def prove_from_inputs_batch(prog: Prog, inputs_list: Sequence[Sequence[int]], proving_key, rng, device: int = 0, lib=None):
+    """K input sets -> K proofs with the assignments resident on the device (zkb_prog_prove_batch).  (r, s) are drawn proof
+    after proof, so the result equals `[prove_from_inputs(prog, x, proving_key, rng) for x in inputs_list]` on the same rng
+    state.  Same failures as prove_from_inputs; an unsatisfied set raises UnsatisfiedConstraint naming it."""
+    from . import backend
+    from .proof import Proof
+    from .rng import fr_rand
+    c = _curve(prog.curve)
+    for x in inputs_list:
+        if len(x) != len(prog.arguments):
+            raise ValueError(f"WrongInputCount: expected {len(prog.arguments)}, received {len(x)}")
+    if not inputs_list:
+        return []
+    pk_bytes = proving_key.read() if hasattr(proving_key, "read") else bytes(proving_key)
+    rs, ss = [], []
+    for _ in inputs_list:
+        rs.append(fr_rand(c, rng))
+        ss.append(fr_rand(c, rng))
+    ctx = backend.context(c, device, lib)
+    with ctx.lock:
+        h, _ = _load_program(ctx, prog)
+        pk_h = None
+        try:
+            pk_h = ctx.pk_load(pk_bytes, 0, 1)
+            res, first = ctx.prog_prove_batch(h, pk_h, [[int(v) % c.r for v in x] for x in inputs_list], rs, ss)
+        finally:
+            if pk_h:
+                ctx.pk_free(pk_h)
+            ctx.prog_free(h)
+    _raise_first_failure(first)
+    return [Proof.from_raw(c, raw, public) for raw, public in res]
