@@ -15,6 +15,7 @@
  *   - ark-poly Radix2EvaluationDomain fft / ifft / coset variants
  *   - ark-groth16 LibsnarkReduction::witness_map and create_proof_with_reduction
  *   - ark-serialize ProvingKey::deserialize_unchecked layout
+ *   - GM17's square arithmetic program at tau and its trapdoor-predicted proof (restating oracle/gm17.py)
  * Parity status: field arithmetic and formats pinned by the reference's KATs via the python oracle
  * (tests/test_oracle_pins.py cross-checks this file against it); proof values "parity unpinned"
  * (no golden proof exists in the reference) — validated by the pairing/trapdoor checks in oracle/ark.py.
@@ -685,6 +686,57 @@ EXPORT int zko_groth16_setup(int curve, uint64_t N, uint64_t ni, uint64_t nw, co
   return (uint64_t)(o - pk_out) == total ? 0 : 6;
 }
 
+/* ------------------------------------------------------------------------------------------- Lagrange coefficients
+ * u[j] = L_j(tau) = Z(tau)/n * w^j / (tau - w^j) over the domain of size 2^lg (closed form, NOT an inverse FFT), and
+ * zt = Z(tau) = tau^n - 1, all Montgomery.  Chunked over the pool: per chunk w^j by one exponentiation and a running product,
+ * one inversion per chunk (Montgomery's trick).  Returns 0, or 3 if tau lies in the domain. */
+static int lagrange_at_tau(const curve_t* c, int lg, const fe* tau, fe* u, fe* zt_out) {
+  const fctx* f = &c->fr;
+  const size_t n = (size_t)1 << lg;
+  fe w; domain_omega(c, lg, &w);
+  fe zt = *tau; for (int i = 0; i < lg; i++) fe_sqr(f, &zt, &zt);
+  fe_sub(f, &zt, &zt, &f->r1);
+  *zt_out = zt;
+  fe nn, ninv, scale; fe_from_u64(f, &nn, n); fe_inv(f, &ninv, &nn); fe_mul(f, &scale, &zt, &ninv);
+  fe* pre = (fe*)malloc(n * sizeof(fe));
+  const int nt = zko_pool_threads();
+  const size_t chunk = (n + nt - 1) / nt;
+  int bad = 0;
+#pragma omp parallel for schedule(static) num_threads(nt)
+  for (int t = 0; t < nt; t++) {
+    size_t lo = (size_t)t * chunk, hi = lo + chunk < n ? lo + chunk : n;
+    if (lo >= hi) continue;
+    uint64_t e[1] = {lo};
+    fe wj; fe_pow(f, &wj, &w, e, 1);
+    fe run = f->r1;
+    for (size_t j = lo; j < hi; j++) {              /* u[j] = w^j (kept), pre[j] = prod_{k<j} (tau - w^k) */
+      fe d; fe_sub(f, &d, tau, &wj);
+      if (fe_is_zero(f, &d)) { bad = 1; d = f->r1; }
+      u[j] = wj; pre[j] = run;
+      fe_mul(f, &run, &run, &d);
+      fe_mul(f, &wj, &wj, &w);
+    }
+    fe inv; fe_inv(f, &inv, &run);
+    for (size_t j = hi; j-- > lo;) {
+      fe d, dinv; fe_sub(f, &d, tau, &u[j]);
+      fe_mul(f, &dinv, &inv, &pre[j]);              /* 1 / (tau - w^j) */
+      fe_mul(f, &inv, &inv, &d);
+      fe_mul(f, &u[j], &u[j], &dinv);
+      fe_mul(f, &u[j], &u[j], &scale);
+    }
+  }
+  free(pre);
+  return bad ? 3 : 0;
+}
+
+/* g1 = g1_k G1, g2 = g2_k G2 (the generators a key made from this trapdoor uses) */
+static void key_generators(int curve, const curve_t* c, const uint64_t* g1_k, const uint64_t* g2_k, g1_jac* g1, g2_jac* g2) {
+  g1_aff s1; g2_aff s2; std_generators(curve, c, &s1, &s2);
+  g1_jac j1; g2_jac j2;
+  g1_from_affine(&c->fq, &j1, &s1); g2_from_affine(&c->fq, &j2, &s2);
+  g1_mul(&c->fq, g1, &j1, g1_k, 4); g2_mul(&c->fq, g2, &j2, g2_k, 4);
+}
+
 /* ------------------------------------------------------------------------------------------- trapdoor prediction
  * Expected Groth16 proof (A, B, C) for a key made by zko_groth16_setup / zkb_groth16_setup from the SAME explicit
  * trapdoor, computed with Fr arithmetic only plus one scalar multiplication of the generator per proof element —
@@ -712,41 +764,10 @@ EXPORT int zko_trapdoor_expected(int curve, uint64_t N, uint64_t ni, uint64_t nw
   read_fr(c, &alpha, trapdoor7); read_fr(c, &beta, trapdoor7 + 4); read_fr(c, &delta, trapdoor7 + 12); read_fr(c, &tau, trapdoor7 + 16);
   memcpy(gk[0], trapdoor7 + 20, 32); memcpy(gk[1], trapdoor7 + 24, 32);
   read_fr(c, &rr, r_s); read_fr(c, &ss, s_s);
-  /* Lagrange coefficients at tau, chunked: per chunk w^j by one exponentiation + running product, one inversion (Montgomery's trick) */
-  fe w; domain_omega(c, lg, &w);
-  fe zt = tau; for (int i = 0; i < lg; i++) fe_sqr(f, &zt, &zt);
-  fe_sub(f, &zt, &zt, &f->r1);
-  fe nn, ninv, scale; fe_from_u64(f, &nn, n); fe_inv(f, &ninv, &nn); fe_mul(f, &scale, &zt, &ninv);
   fe* u = (fe*)malloc(n * sizeof(fe));
-  fe* pre = (fe*)malloc(n * sizeof(fe));
+  fe zt;
+  if (lagrange_at_tau(c, lg, &tau, u, &zt)) { free(u); return 3; }
   const int nt = zko_pool_threads();
-  const size_t chunk = (n + nt - 1) / nt;
-  int bad = 0;
-#pragma omp parallel for schedule(static) num_threads(nt)
-  for (int t = 0; t < nt; t++) {
-    size_t lo = (size_t)t * chunk, hi = lo + chunk < n ? lo + chunk : n;
-    if (lo >= hi) continue;
-    uint64_t e[1] = {lo};
-    fe wj; fe_pow(f, &wj, &w, e, 1);
-    fe run = f->r1;
-    for (size_t j = lo; j < hi; j++) {              /* u[j] = w^j (kept), pre[j] = prod_{k<j} (tau - w^k) */
-      fe d; fe_sub(f, &d, &tau, &wj);
-      if (fe_is_zero(f, &d)) { bad = 1; d = f->r1; }
-      u[j] = wj; pre[j] = run;
-      fe_mul(f, &run, &run, &d);
-      fe_mul(f, &wj, &wj, &w);
-    }
-    fe inv; fe_inv(f, &inv, &run);
-    for (size_t j = hi; j-- > lo;) {
-      fe d, dinv; fe_sub(f, &d, &tau, &u[j]);
-      fe_mul(f, &dinv, &inv, &pre[j]);              /* 1 / (tau - w^j) */
-      fe_mul(f, &inv, &inv, &d);
-      fe_mul(f, &u[j], &u[j], &dinv);
-      fe_mul(f, &u[j], &u[j], &scale);
-    }
-  }
-  free(pre);
-  if (bad) { free(u); return 3; }
   fe* zm = load_z(c, z, m);
   const uint64_t* rp[3] = {a_rowptr, b_rowptr, c_rowptr}; const uint32_t* cl[3] = {a_col, b_col, c_col}; const uint64_t* vl[3] = {a_val, b_val, c_val};
   fe all[3], inst[3];
@@ -793,11 +814,178 @@ EXPORT int zko_trapdoor_expected(int curve, uint64_t N, uint64_t ni, uint64_t nw
   fe_mul(f, &t1, &rr, &bd); fe_add(f, &cd, &cd, &t1);
   fe_mul(f, &t1, &rr, &ss); fe_mul(f, &t1, &t1, &delta); fe_sub(f, &cd, &cd, &t1);
   fe ac, bc, cc; fe_from_mont(f, &ac, &ad); fe_from_mont(f, &bc, &bd); fe_from_mont(f, &cc, &cd);
-  g1_aff s1; g2_aff s2; std_generators(curve, c, &s1, &s2);
-  g1_jac j1, g1, pa1, pc1; g2_jac j2, g2, pb2;
-  g1_from_affine(&c->fq, &j1, &s1); g2_from_affine(&c->fq, &j2, &s2);
-  g1_mul(&c->fq, &g1, &j1, gk[0], 4); g2_mul(&c->fq, &g2, &j2, gk[1], 4);
+  g1_jac g1, pa1, pc1; g2_jac g2, pb2;
+  key_generators(curve, c, gk[0], gk[1], &g1, &g2);
   g1_mul(&c->fq, &pa1, &g1, ac.l, 4); g2_mul(&c->fq, &pb2, &g2, bc.l, 4); g1_mul(&c->fq, &pc1, &g1, cc.l, 4);
+  g1_aff oa, oc; g2_aff ob;
+  g1_to_affine(&c->fq, &oa, &pa1); g2_to_affine(&c->fq, &ob, &pb2); g1_to_affine(&c->fq, &oc, &pc1);
+  g1_write(c, proof_out, &oa); g2_write(c, proof_out + g1b, &ob); g1_write(c, proof_out + g1b + g2b, &oc);
+  return 0;
+}
+
+/* ------------------------------------------------------------------------------------------- GM17 (Groth-Maller 2017)
+ * The square arithmetic program of ark-gm17's R1CStoSAP (restated in oracle/gm17.py): R1CS row i becomes SAP rows 2i, 2i + 1
+ *   (A_i + B_i)^2 = 4 C_i + x_i,   (A_i - B_i)^2 = x_i,     x_i = (A_i z - B_i z)^2 at SAP column m + i,
+ * then the constant row e = 2N (1^2 = 1) and per public input j >= 1 rows e + 2j - 1, e + 2j
+ *   (z_j + 1)^2 = 4 z_j + y_j,     (z_j - 1)^2 = y_j,       y_j = (z_j - 1)^2 at SAP column m + N - 1 + j,
+ * over a domain of n = 2^lg >= 2N + 2(ni - 1) + 1 points; nv = m + N + ni - 1 SAP variables (the constant included).
+ * trapdoor6 = alpha, beta, gamma, tau, g1_k, g2_k (canonical LE). */
+static void gm17_domain(uint64_t N, uint64_t ni, size_t* n, int* lg) {
+  const uint64_t rows = 2 * N + 2 * (ni - 1) + 1;
+  *n = 1; *lg = 0;
+  while (*n < rows) { *n <<= 1; (*lg)++; }
+}
+
+/* <M_row, z> over all columns and over the instance columns (< ni) alone */
+static void row_dot(const curve_t* c, const r1cs_t* r, int k, uint64_t row, const fe* zm, fe* all, fe* inst) {
+  const fctx* f = &c->fr;
+  memset(all, 0, sizeof *all); memset(inst, 0, sizeof *inst);
+  for (uint64_t e = r->rowptr[k][row]; e < r->rowptr[k][row + 1]; e++) {
+    fe v, p; read_fr(c, &v, r->val[k] + 4 * e);
+    fe_mul(f, &p, &v, &zm[r->col[k][e]]);
+    fe_add(f, all, all, &p);
+    if (r->col[k][e] < r->ni) fe_add(f, inst, inst, &p);
+  }
+}
+
+/* u_i(tau) ("a") and w_i(tau) ("c") of every SAP variable (canonical, nv x 4 limbs each) and Z(tau): R1CStoSAP's
+ * instance_map_with_evaluation, with the Lagrange coefficients in closed form.  Returns 0, or 3 if tau lies in the domain. */
+EXPORT int zko_gm17_sap_at_tau(int curve, uint64_t N, uint64_t ni, uint64_t nw, const uint64_t* a_rowptr, const uint32_t* a_col,
+                               const uint64_t* a_val, const uint64_t* b_rowptr, const uint32_t* b_col, const uint64_t* b_val,
+                               const uint64_t* c_rowptr, const uint32_t* c_col, const uint64_t* c_val, const uint64_t* tau_s,
+                               uint64_t* a_out, uint64_t* c_out, uint64_t* zt_out) {
+  curves_init();
+  const curve_t* c = &CURVES[curve];
+  const fctx* f = &c->fr;
+  const uint64_t m = ni + nw, nv = m + N + ni - 1, e_off = 2 * N;
+  size_t n; int lg; gm17_domain(N, ni, &n, &lg);
+  fe tau, zt; read_fr(c, &tau, tau_s);
+  fe* u = (fe*)malloc(n * sizeof(fe));
+  if (lagrange_at_tau(c, lg, &tau, u, &zt)) { free(u); return 3; }
+  fe* a = (fe*)calloc(nv, sizeof(fe)); fe* cc = (fe*)calloc(nv, sizeof(fe));
+  const uint64_t* rp[3] = {a_rowptr, b_rowptr, c_rowptr}; const uint32_t* cl[3] = {a_col, b_col, c_col}; const uint64_t* vl[3] = {a_val, b_val, c_val};
+  for (uint64_t row = 0; row < N; row++) {
+    fe w[3];
+    fe_add(f, &w[0], &u[2 * row], &u[2 * row + 1]);              /* A: u_2i + u_2i+1 */
+    fe_sub(f, &w[1], &u[2 * row], &u[2 * row + 1]);              /* B: u_2i - u_2i+1 */
+    fe_dbl(f, &w[2], &u[2 * row]); fe_dbl(f, &w[2], &w[2]);      /* C: 4 u_2i */
+    for (int k = 0; k < 3; k++) {
+      fe* dst = k == 2 ? cc : a;
+      for (uint64_t e = rp[k][row]; e < rp[k][row + 1]; e++) {
+        fe v, p; read_fr(c, &v, vl[k] + 4 * e); fe_mul(f, &p, &v, &w[k]); fe_add(f, &dst[cl[k][e]], &dst[cl[k][e]], &p);
+      }
+    }
+    fe_add(f, &cc[m + row], &cc[m + row], &w[0]);                /* x_i */
+  }
+  fe_add(f, &a[0], &a[0], &u[e_off]); fe_add(f, &cc[0], &cc[0], &u[e_off]);
+  for (uint64_t j = 1; j < ni; j++) {
+    const fe* u1 = &u[e_off + 2 * j - 1]; const fe* u2 = &u[e_off + 2 * j];
+    fe s, d, q; fe_add(f, &s, u1, u2); fe_sub(f, &d, u1, u2); fe_dbl(f, &q, u1); fe_dbl(f, &q, &q);
+    fe_add(f, &a[j], &a[j], &s); fe_add(f, &a[0], &a[0], &d);
+    fe_add(f, &cc[j], &cc[j], &q); fe_add(f, &cc[m + N - 1 + j], &cc[m + N - 1 + j], &s);
+  }
+  for (uint64_t i = 0; i < nv; i++) {
+    fe t; fe_from_mont(f, &t, &a[i]); memcpy(a_out + 4 * i, t.l, 32);
+    fe_from_mont(f, &t, &cc[i]); memcpy(c_out + 4 * i, t.l, 32);
+  }
+  fe t; fe_from_mont(f, &t, &zt); memcpy(zt_out, t.l, 32);
+  free(u); free(a); free(cc);
+  return 0;
+}
+
+/* Expected GM17 proof (A, B, C) for a key made by zkb_gm17_setup from the SAME explicit trapdoor, with Fr arithmetic and three
+ * generator multiplications — no NTT, no MSM, no key (restates oracle/gm17.py::trapdoor_expected_proof; Groth-Maller Fig. 4 with
+ * a(x) masked by d1 Z and c(x) by d2 Z):
+ *   a0    = sum_i u_i(tau) s_i,  c0 = sum_i w_i(tau) s_i     over the full SAP assignment s = [z | x | y]
+ *           (per R1CS row: (u_2i + u_2i+1) A_i z + (u_2i - u_2i+1) B_i z, and 4 u_2i C_i z + (u_2i + u_2i+1) x_i; then the extra rows)
+ *   at    = a0 + d1 Z,  ct = c0 + d2 Z,  ht = (at^2 - ct) / Z
+ *   aux   = sum_(i >= ni) (gamma^2 w_i + (alpha + beta) gamma u_i) s_i       (a0, c0 minus their instance-column parts)
+ *   A     = gamma (at + r Z) g1,  B = the same dlog times g2
+ *   C     = [aux + d1 (alpha + beta) gamma Z + d2 gamma^2 Z + r^2 gamma^2 Z^2 + r (alpha + beta) gamma Z + gamma^2 Z (ht + 2 r at)] g1
+ * Returns 0, or 3 if tau lies in the SAP domain. */
+EXPORT int zko_gm17_trapdoor_expected(int curve, uint64_t N, uint64_t ni, uint64_t nw, const uint64_t* a_rowptr, const uint32_t* a_col,
+                                      const uint64_t* a_val, const uint64_t* b_rowptr, const uint32_t* b_col, const uint64_t* b_val,
+                                      const uint64_t* c_rowptr, const uint32_t* c_col, const uint64_t* c_val, const uint64_t* trapdoor6,
+                                      const uint64_t* z, const uint64_t* d1_s, const uint64_t* d2_s, const uint64_t* r_s,
+                                      uint8_t* proof_out) {
+  curves_init();
+  const curve_t* c = &CURVES[curve];
+  const fctx* f = &c->fr;
+  const int g1b = 2 * c->fq_bytes, g2b = 4 * c->fq_bytes;
+  const uint64_t m = ni + nw, e_off = 2 * N;
+  size_t n; int lg; gm17_domain(N, ni, &n, &lg);
+  fe alpha, beta, gamma, tau, d1, d2, rr;
+  read_fr(c, &alpha, trapdoor6); read_fr(c, &beta, trapdoor6 + 4); read_fr(c, &gamma, trapdoor6 + 8); read_fr(c, &tau, trapdoor6 + 12);
+  read_fr(c, &d1, d1_s); read_fr(c, &d2, d2_s); read_fr(c, &rr, r_s);
+  fe* u = (fe*)malloc(n * sizeof(fe));
+  fe zt;
+  if (lagrange_at_tau(c, lg, &tau, u, &zt)) { free(u); return 3; }
+  fe* zm = load_z(c, z, m);
+  r1cs_t r = {N, ni, nw, {a_rowptr, b_rowptr, c_rowptr}, {a_col, b_col, c_col}, {a_val, b_val, c_val}};
+  /* per-row sums: [0] a0, [1] a0 over instance columns, [2] c0, [3] c0 over instance columns; per-thread partials */
+  const int nt = zko_pool_threads();
+  fe* part = (fe*)calloc(4 * (size_t)nt, sizeof(fe));
+  const size_t rchunk = (N + nt - 1) / nt;
+#pragma omp parallel for schedule(static) num_threads(nt)
+  for (int t = 0; t < nt; t++) {
+    size_t lo = (size_t)t * rchunk, hi = lo + rchunk < N ? lo + rchunk : N;
+    fe s[4]; memset(s, 0, sizeof s);
+    for (size_t row = lo; row < hi; row++) {
+      fe az, azi, bz, bzi, cz, czi, ua, us, u4, x, p;
+      row_dot(c, &r, 0, row, zm, &az, &azi); row_dot(c, &r, 1, row, zm, &bz, &bzi); row_dot(c, &r, 2, row, zm, &cz, &czi);
+      fe_add(f, &ua, &u[2 * row], &u[2 * row + 1]); fe_sub(f, &us, &u[2 * row], &u[2 * row + 1]);
+      fe_dbl(f, &u4, &u[2 * row]); fe_dbl(f, &u4, &u4);
+      fe_mul(f, &p, &ua, &az); fe_add(f, &s[0], &s[0], &p); fe_mul(f, &p, &us, &bz); fe_add(f, &s[0], &s[0], &p);
+      fe_mul(f, &p, &ua, &azi); fe_add(f, &s[1], &s[1], &p); fe_mul(f, &p, &us, &bzi); fe_add(f, &s[1], &s[1], &p);
+      fe_sub(f, &x, &az, &bz); fe_sqr(f, &x, &x);
+      fe_mul(f, &p, &u4, &cz); fe_add(f, &s[2], &s[2], &p); fe_mul(f, &p, &ua, &x); fe_add(f, &s[2], &s[2], &p);
+      fe_mul(f, &p, &u4, &czi); fe_add(f, &s[3], &s[3], &p);
+    }
+    for (int k = 0; k < 4; k++) part[4 * t + k] = s[k];
+  }
+  fe a0, ai, c0, ci, p;
+  memset(&a0, 0, sizeof a0); memset(&ai, 0, sizeof ai); memset(&c0, 0, sizeof c0); memset(&ci, 0, sizeof ci);
+  for (int t = 0; t < nt; t++) {
+    fe_add(f, &a0, &a0, &part[4 * t]); fe_add(f, &ai, &ai, &part[4 * t + 1]);
+    fe_add(f, &c0, &c0, &part[4 * t + 2]); fe_add(f, &ci, &ci, &part[4 * t + 3]);
+  }
+  free(part);
+  /* the extra rows: every column they touch is an instance column except y_j's */
+  fe_mul(f, &p, &u[e_off], &zm[0]);
+  fe_add(f, &a0, &a0, &p); fe_add(f, &ai, &ai, &p); fe_add(f, &c0, &c0, &p); fe_add(f, &ci, &ci, &p);
+  for (uint64_t j = 1; j < ni; j++) {
+    const fe* u1 = &u[e_off + 2 * j - 1]; const fe* u2 = &u[e_off + 2 * j];
+    fe s, d, q, y;
+    fe_add(f, &s, u1, u2); fe_sub(f, &d, u1, u2); fe_dbl(f, &q, u1); fe_dbl(f, &q, &q);
+    fe_sub(f, &y, &zm[j], &f->r1); fe_sqr(f, &y, &y);
+    fe ta; fe_mul(f, &ta, &s, &zm[j]); fe_mul(f, &p, &d, &zm[0]); fe_add(f, &ta, &ta, &p);
+    fe_add(f, &a0, &a0, &ta); fe_add(f, &ai, &ai, &ta);
+    fe tc; fe_mul(f, &tc, &q, &zm[j]);
+    fe_add(f, &c0, &c0, &tc); fe_add(f, &ci, &ci, &tc);
+    fe_mul(f, &p, &s, &y); fe_add(f, &c0, &c0, &p);
+  }
+  free(u); free(zm);
+  fe ab, g2, abg, at, ct, ht, zinv, aux, t1, t2;
+  fe_add(f, &ab, &alpha, &beta); fe_sqr(f, &g2, &gamma); fe_mul(f, &abg, &ab, &gamma);
+  fe_mul(f, &t1, &d1, &zt); fe_add(f, &at, &a0, &t1);
+  fe_mul(f, &t1, &d2, &zt); fe_add(f, &ct, &c0, &t1);
+  fe_inv(f, &zinv, &zt);
+  fe_sqr(f, &ht, &at); fe_sub(f, &ht, &ht, &ct); fe_mul(f, &ht, &ht, &zinv);
+  fe_sub(f, &t1, &c0, &ci); fe_mul(f, &aux, &g2, &t1);
+  fe_sub(f, &t1, &a0, &ai); fe_mul(f, &t1, &abg, &t1); fe_add(f, &aux, &aux, &t1);
+  fe adl, cdl;
+  fe_mul(f, &t1, &rr, &zt); fe_add(f, &t1, &at, &t1); fe_mul(f, &adl, &gamma, &t1);         /* gamma (at + r Z) */
+  cdl = aux;
+  fe_mul(f, &t1, &d1, &abg); fe_mul(f, &t1, &t1, &zt); fe_add(f, &cdl, &cdl, &t1);
+  fe_mul(f, &t1, &d2, &g2); fe_mul(f, &t1, &t1, &zt); fe_add(f, &cdl, &cdl, &t1);
+  fe_sqr(f, &t1, &rr); fe_mul(f, &t1, &t1, &g2); fe_mul(f, &t1, &t1, &zt); fe_mul(f, &t1, &t1, &zt); fe_add(f, &cdl, &cdl, &t1);
+  fe_mul(f, &t1, &rr, &abg); fe_mul(f, &t1, &t1, &zt); fe_add(f, &cdl, &cdl, &t1);
+  fe_mul(f, &t2, &rr, &at); fe_dbl(f, &t2, &t2); fe_add(f, &t2, &t2, &ht);
+  fe_mul(f, &t1, &g2, &zt); fe_mul(f, &t1, &t1, &t2); fe_add(f, &cdl, &cdl, &t1);
+  fe ac, cc; fe_from_mont(f, &ac, &adl); fe_from_mont(f, &cc, &cdl);
+  g1_jac g1, pa1, pc1; g2_jac g2g, pb2;
+  key_generators(curve, c, trapdoor6 + 16, trapdoor6 + 20, &g1, &g2g);
+  g1_mul(&c->fq, &pa1, &g1, ac.l, 4); g2_mul(&c->fq, &pb2, &g2g, ac.l, 4); g1_mul(&c->fq, &pc1, &g1, cc.l, 4);
   g1_aff oa, oc; g2_aff ob;
   g1_to_affine(&c->fq, &oa, &pa1); g2_to_affine(&c->fq, &ob, &pb2); g1_to_affine(&c->fq, &oc, &pc1);
   g1_write(c, proof_out, &oa); g2_write(c, proof_out + g1b, &ob); g1_write(c, proof_out + g1b + g2b, &oc);

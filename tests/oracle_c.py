@@ -104,3 +104,39 @@ class OracleC:
         if rc != 0:
             raise RuntimeError(f"zko_trapdoor_expected rc={rc}")
         return out.tobytes()
+
+    @staticmethod
+    def _sizes(r1cs):
+        return C.c_uint64(r1cs.num_constraints), C.c_uint64(r1cs.num_instance), C.c_uint64(r1cs.num_witness)
+
+    def gm17_trapdoor_expected(self, curve, r1cs, trapdoor6, z, d1: int, d2: int, r: int, fq_bytes):
+        """Expected GM17 proof bytes from the trapdoor (alpha, beta, gamma, tau, g1_k, g2_k) and the masks d1, d2, r: Fr
+        arithmetic + three generator multiplications (no NTT / MSM / key)."""
+        from zokrates_b200._lib import fr_array
+        td = fr_array(trapdoor6)
+        z = np.ascontiguousarray(z, dtype=np.uint64)
+        masks = fr_array([d1, d2, r])
+        out = np.zeros(8 * fq_bytes, dtype=np.uint8)
+        args, keep = self._mats(r1cs)
+        rc = self.dll.zko_gm17_trapdoor_expected(curve, *self._sizes(r1cs), *args, C.c_void_p(td.ctypes.data),
+                                                 C.c_void_p(z.ctypes.data), C.c_void_p(masks[0].ctypes.data),
+                                                 C.c_void_p(masks[1].ctypes.data), C.c_void_p(masks[2].ctypes.data),
+                                                 C.c_void_p(out.ctypes.data))
+        if rc != 0:
+            raise RuntimeError(f"zko_gm17_trapdoor_expected rc={rc}")
+        return out.tobytes()
+
+    def gm17_sap_at_tau(self, curve, r1cs, tau: int):
+        """(u_i(tau), w_i(tau)) of every SAP variable as two (nv, 4) canonical limb arrays, and Z(tau) as an int."""
+        from zokrates_b200._lib import fr_array, fr_from_array
+        nv = r1cs.num_instance + r1cs.num_witness + r1cs.num_constraints + r1cs.num_instance - 1
+        a = np.zeros((nv, 4), dtype=np.uint64)
+        cc = np.zeros((nv, 4), dtype=np.uint64)
+        zt = np.zeros((1, 4), dtype=np.uint64)
+        ta = fr_array([tau])
+        args, keep = self._mats(r1cs)
+        rc = self.dll.zko_gm17_sap_at_tau(curve, *self._sizes(r1cs), *args, C.c_void_p(ta.ctypes.data), C.c_void_p(a.ctypes.data),
+                                          C.c_void_p(cc.ctypes.data), C.c_void_p(zt.ctypes.data))
+        if rc != 0:
+            raise RuntimeError(f"zko_gm17_sap_at_tau rc={rc}")
+        return a, cc, fr_from_array(zt)[0]

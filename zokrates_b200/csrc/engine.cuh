@@ -2072,8 +2072,16 @@ class Engine : public EngineBase {
     gc = HG1X::add(gc, sum.h);
     HG1A pc = HG1X::to_affine(gc);
     HG2A pb = fut_pb.get();
-    auto put = [&](size_t slot, const HFq& v) { HFq c = HFq::from_mont(v); memcpy(proof_out + slot * FQB, c.v, FQB); };
+    write_proof(proof_out, pa, pb, pc);
+  }
+  // A | B | C in ark's uncompressed encoding: canonical affine coordinates, and the point at infinity as zero coordinates with
+  // the infinity flag (bit 6 of the point's last byte)
+  static void write_proof(uint8_t* out, const HG1A& pa, const HG2A& pb, const HG1A& pc) {
+    auto put = [&](size_t slot, const HFq& v) { HFq c = HFq::from_mont(v); memcpy(out + slot * FQB, c.v, FQB); };
     put(0, pa.x); put(1, pa.y); put(2, pb.x.c0); put(3, pb.x.c1); put(4, pb.y.c0); put(5, pb.y.c1); put(6, pc.x); put(7, pc.y);
+    if (pa.is_inf()) out[G1B - 1] |= 0x40;
+    if (pb.is_inf()) out[G1B + G2B - 1] |= 0x40;
+    if (pc.is_inf()) out[2 * G1B + G2B - 1] |= 0x40;
   }
 
   // Multi-GPU: the rank that will finalize may announce (pk, r, s) before it starts its own share of the proof; the four

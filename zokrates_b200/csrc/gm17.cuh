@@ -211,8 +211,7 @@ void Engine<C>::gm17_prove(uint64_t pkh, uint64_t rh, const uint64_t* z, const u
   gc = HG1X::add(gc, s_h);
   const HG1A pa = HG1X::to_affine(ga), pcc = HG1X::to_affine(gc);
   const HG2A pb = HG2X::to_affine(gb);
-  auto put = [&](size_t slot, const HFq& v) { HFq c = HFq::from_mont(v); memcpy(proof_out + slot * FQB, c.v, FQB); };
-  put(0, pa.x); put(1, pa.y); put(2, pb.x.c0); put(3, pb.x.c1); put(4, pb.y.c0); put(5, pb.y.c1); put(6, pcc.x); put(7, pcc.y);
+  write_proof(proof_out, pa, pb, pcc);
 }
 
 // ---- circuit-specific GM17 setup from an explicit trapdoor (alpha, beta, gamma, tau, g1_k, g2_k) ---------------------------------
