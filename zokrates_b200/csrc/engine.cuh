@@ -617,17 +617,36 @@ class Engine : public EngineBase {
     // filled by msm_tail: the bit-sum reduction consumed `tree_bits` index bits and left `tree_cnt` block totals per window
     uint32_t nt1 = 0;         // chunks of the last accumulation into this workspace (the partial lists hold 2 nt1 entries)
     uint32_t tree_cnt = 1, tree_bits = 0;
-    size_t out_entries = 0;   // XYZZ entries of the result slot the host has to read: (1 + tree_bits) * W * tree_cnt
     void destroy() { if (has_stream) { stream_destroy(tail); has_stream = false; } acc_done.destroy(); tail_done.destroy(); }
   };
+  // The five MSMs of one proof or of one batch pass: h, l, a, b1 (G1) and b2 (G2), in this order in `ws`, in the result slots
+  // and in Partial.  The h plan serves h; the z plan serves l, a, b1 and b2 through its views 0, 1, 2 and 2.
+  struct MsmSet {
+    MsmPlan plan_z, plan_h;
+    MsmWs ws[5];
+    DevBuf<uint8_t> d_win;          // the result slots, packed (msm_slots), so that one copy brings all of them to the host
+    HostBuf hw;                     // pinned landing zone of the same
+    size_t off[6] = {0, 0, 0, 0, 0, 0};   // byte offset of slot k; off[5] is the total
+    const MsmPlan& plan(int k) const { return k ? plan_z : plan_h; }
+    void destroy() { for (auto& w : ws) w.destroy(); }
+    size_t device_bytes() const {
+      size_t b = d_win.bytes();
+      for (const MsmPlan* p : {&plan_z, &plan_h})
+        b += p->digits.bytes() + p->ranks.bytes() + p->counts.bytes() + p->offsets.bytes() + p->sorted.bytes() + p->scan_tmp.bytes() +
+             p->view_tile_cnt.bytes() + p->view_tile_off.bytes() + p->view_pre32.bytes() + p->view_mask32.bytes();
+      for (const MsmWs& w : ws) {
+        b += w.buckets.bytes();
+        for (int k = 0; k < 2; k++) b += w.val[k].bytes() + w.key[k].bytes();
+        for (int k = 0; k < 4; k++) b += w.tree[k].bytes();
+      }
+      return b;
+    }
+  };
   struct ProofSlot {
-    DevBuf<Fr> z_canon, z_mont, a, b, c, h;   // assignment (when it came from the host), its Montgomery image, witness-map vectors
+    DevBuf<Fr> z_canon, z_mont, v, h;         // assignment (when it came from the host), its Montgomery image, chains, h
     const Fr* z_src = nullptr;                // canonical assignment this proof reads (own upload or the resident one)
     bool sparse_z = false;
-    MsmPlan plan_z, plan_h;
-    MsmWs ws[5];                              // h, l, a, b1, b2
-    DevBuf<uint8_t> d_win;                    // result slots of the five MSMs
-    HostBuf hw;                               // pinned landing zone of the same
+    MsmSet msm;
     std::unique_ptr<StageTimer> tm, tm2;
     Event ev_z_ready, ev_h_ready, ev_chains_done, ev_exchange, ev_plan_z, done;
     Stream fin; bool has_fin = false;         // waits for the five tails and copies the results out, off the main stream
@@ -637,7 +656,7 @@ class Engine : public EngineBase {
     uint32_t r[8], s[8];
     std::future<FixedMults> fm;
     void destroy() {
-      for (auto& w : ws) w.destroy();
+      msm.destroy();
       ev_z_ready.destroy(); ev_h_ready.destroy(); ev_chains_done.destroy(); ev_exchange.destroy(); ev_plan_z.destroy(); done.destroy();
       if (has_fin) { stream_destroy(fin); has_fin = false; }
     }
@@ -648,42 +667,58 @@ class Engine : public EngineBase {
   void slot_vectors(ProofSlot& sl, const R1cs& r) {
     const size_t n = (size_t)1 << r.log_n;
     sl.z_canon.ensure(r.m); sl.z_mont.ensure(r.m);
-    sl.a.ensure(n); sl.b.ensure(n); sl.c.ensure(n); sl.h.ensure(n);
+    sl.v.ensure(3 * n); sl.h.ensure(n);
   }
 
   // h (canonical, natural order) = witness_map(z)   [device-resident]
   // The witness map in two halves so that several GPUs can share it (zkb_groth16_prove_begin / _end):
-  //   chains: for every k in `mask`: v_k = coset_fft(ifft(M_k z)) — three independent SpMV + 2 transforms (a, b, c)
-  //   finish: h = coset_ifft((a∘b − c) / Z)  — needs all three chains
-  void wm_chains(R1cs& r, ProofSlot& sl, uint32_t mask, StageTimer& tm) {
+  //   chains: v_k = coset_fft(ifft(M_k z)) for the matrices k = A, B, C — three independent SpMV + 2 transforms
+  //   finish: h = coset_ifft((v_A ∘ v_B − v_C) / Z)  — needs all three chains
+  // The chains of `count` proofs lie in one buffer: chain k of proof j at (k count + j) n.
+
+  // M_k z for the matrices k_lo <= k < k_hi and K assignments (zm: interleaved Montgomery z, z[col * K + j]) in one launch, out
+  // as the chains above: rows below N the products, then the instance variables in the A chain, zeros up to n.  n = N gives
+  // the products alone.  G assignments per thread.
+  template <int G>
+  void spmv(const R1cs& r, const Fr* zm, uint32_t K, Fr* out, size_t n, uint32_t k_lo, uint32_t k_hi) {
+    const uint32_t* rpA = r.rowptr[0].p; const uint32_t* clA = r.col[0].p; const Fr* vlA = r.val[0].p;
+    const uint32_t* rpB = r.rowptr[1].p; const uint32_t* clB = r.col[1].p; const Fr* vlB = r.val[1].p;
+    const uint32_t* rpC = r.rowptr[2].p; const uint32_t* clC = r.col[2].p; const Fr* vlC = r.val[2].p;
+    const uint32_t N = (uint32_t)r.N, ni = (uint32_t)r.ni, ngroups = (K + G - 1) / G;
+    // thread (matrix, group of assignments, row): the row index runs fastest, so the output stores are coalesced
+    launch<k_spmv>(st_, (size_t)(k_hi - k_lo) * ngroups * n, ZKB_LAMBDA(size_t t) {
+      const uint32_t row = (uint32_t)(t % n), q = (uint32_t)(t / n), kind = k_lo + q / ngroups, g = q % ngroups;
+      const uint32_t* rp = kind == 0 ? rpA : kind == 1 ? rpB : rpC;
+      const uint32_t* cl = kind == 0 ? clA : kind == 1 ? clB : clC;
+      const Fr* vl = kind == 0 ? vlA : kind == 1 ? vlB : vlC;
+      spmv_batch_body<Fr, G>(rp, cl, vl, zm, K, g * G, out + (size_t)kind * K * n, n, N, kind == 0 ? ni : 0, row);
+    });
+  }
+  // chains k_lo <= k < k_hi of K proofs: one SpMV launch, then the transforms of their (k_hi - k_lo) K vectors
+  void wm_chains(const R1cs& r, const Fr* zm, uint32_t K, Fr* v, uint32_t k_lo, uint32_t k_hi) {
     DomainT& d = domain(r.log_n);
     const uint32_t lg = r.log_n;
     const size_t n = (size_t)1 << lg;
+    if (K == 1) spmv<1>(r, zm, K, v, n, k_lo, k_hi);
+    else spmv<SPMV_GROUP>(r, zm, K, v, n, k_lo, k_hi);
+    Fr* x = v + (size_t)k_lo * K * n;
+    ntt_dif(x, d.tw_inv.p, lg, (k_hi - k_lo) * K);
+    ntt_dit(x, d.tw_fwd.p, lg, d.cos_fwd.p, (k_hi - k_lo) * K);   // coset shift (g^k / n at the bit-reversed position) fused into the first pass
+  }
+  // the chains of `mask` of one proof, one SpMV and one transform set each
+  void slot_chains(R1cs& r, ProofSlot& sl, uint32_t mask, StageTimer& tm) {
     tm.begin("witness_map_chains");
     convert(sl.z_src, sl.z_mont.p, 0, r.m);
-    Fr* vec[3] = {sl.a.p, sl.b.p, sl.c.p};
-    const Fr* zm = sl.z_mont.p;
-    const Fr* t1 = d.cos_fwd.p;
-    for (int k = 0; k < 3; k++) {
-      if (!((mask >> k) & 1u)) continue;
-      Fr* out = vec[k];
-      const uint32_t* rp = r.rowptr[k].p;
-      const uint32_t* cl = r.col[k].p;
-      const Fr* vl = r.val[k].p;
-      const uint32_t N = (uint32_t)r.N;
-      dev_zero(st_, out + r.N, (n - r.N) * FRB);
-      launch<k_spmv>(st_, r.N, ZKB_LAMBDA(size_t t) { spmv_body<Fr>(rp, cl, vl, zm, out, N, (uint32_t)t); });
-      if (k == 0) d2d(st_, sl.a.p + r.N, sl.z_mont.p, r.ni * FRB);  // a[N + j] = z[j] for the instance variables
-      ntt_dif(out, d.tw_inv.p, lg);
-      ntt_dit(out, d.tw_fwd.p, lg, t1);   // coset shift (g^k / n at the bit-reversed position) fused into the first pass
-    }
+    for (uint32_t k = 0; k < 3; k++)
+      if ((mask >> k) & 1u) wm_chains(r, sl.z_mont.p, 1, sl.v.p, k, k + 1);
     tm.end();
   }
-  // `count` proofs: vector k of a, b, c and h at offset k n (the chains of a batch are back to back)
-  void wm_finish(R1cs& r, Fr* pa, const Fr* pb, const Fr* pc, Fr* ph, uint32_t count, StageTimer& tm, const char* name) {
+  // h of `count` proofs (vector j at ph + j n) from their chains
+  void wm_finish(R1cs& r, Fr* v, Fr* ph, uint32_t count, StageTimer& tm, const char* name) {
     DomainT& d = domain(r.log_n);
     const uint32_t lg = r.log_n;
     const size_t cn = (size_t)count << lg;
+    Fr* pa = v; const Fr* pb = v + cn; const Fr* pc = v + 2 * cn;
     tm.begin(name);
     Fr zinv = d.zinv;
     launch<k_qap_pointwise>(st_, cn, ZKB_LAMBDA(size_t t) { qap_pointwise_body<Fr>(pa, pb, pc, zinv, (uint32_t)cn, (uint32_t)t); });
@@ -708,8 +743,8 @@ class Engine : public EngineBase {
     h2d(st_, sl.z_canon.p, z, r.m * FRB);
     sl.z_src = sl.z_canon.p;
     tm.begin("witness_map");
-    wm_chains(r, sl, 7, tm);
-    wm_finish(r, sl.a.p, sl.b.p, sl.c.p, sl.h.p, 1, tm, "witness_map_finish");
+    slot_chains(r, sl, 7, tm);
+    wm_finish(r, sl.v.p, sl.h.p, 1, tm, "witness_map_finish");
     tm.end();
     d2h(st_, h_out, sl.h.p, n * FRB);
     stream_sync(st_);
@@ -1095,19 +1130,18 @@ class Engine : public EngineBase {
     const uint64_t per = n * plan_w(plan_c(n, pre_c)) * nviews;
     return per ? ((1ull << 32) - 1) / per : ~0ull;
   }
+  // the shape plan_build gives an MSM of n pairs per proof and K proofs
+  static MsmShape plan_shape(uint64_t n, uint32_t pre_c, uint32_t K) {
+    const uint32_t c = n ? plan_c(n, pre_c) : 0;
+    return MsmShape{(uint32_t)n, c, c ? plan_w(c) : 0, c ? 1u << (c - 1) : 0, pre_c ? 1u : 0u, K};
+  }
 
   // K > 1: a batch of K scalar vectors, vector k at scalars + k * stride (MsmShape)
   void plan_build(MsmPlan& pl, const Fr* scalars, uint64_t n, uint32_t nviews = 1, const uint8_t* skip = nullptr,
                   uint32_t pre_c = 0 /* != 0: precomputed window tables with this c */, uint32_t K = 1, size_t stride = 0) {
-    pl.sh.n = (uint32_t)n;
-    pl.sh.K = K;
+    pl.sh = plan_shape(n, pre_c, K);
     pl.nviews = nviews;
-    pl.sh.pre = pre_c ? 1 : 0;
     if (n == 0) return;
-    uint32_t c = plan_c(n, pre_c);
-    pl.sh.c = c;
-    pl.sh.W = plan_w(c);
-    pl.sh.B = 1u << (c - 1);
     pl.nbuckets = msm_nbuckets(pl.sh);
     uint64_t total = (uint64_t)K * n * pl.sh.W;
     if (K == 0 || total * nviews >= (1ull << 32)) throw Error(ZKB_E_ARG, "msm too large");
@@ -1281,21 +1315,23 @@ class Engine : public EngineBase {
   // Levels of the device bucket reduction: it stops when a proof's windows hold at most host_nodes block totals, so the host
   // share of every proof is the same whatever the batch size.  Returns the XYZZ entries of the result slot (all K proofs).
   template <class F>
-  size_t tail_levels(const MsmPlan& pl, uint32_t& cnt, uint32_t& nbits) const {
-    const uint32_t Wp = pl.sh.pre ? 1 : pl.sh.W;
+  size_t tail_levels(const MsmShape& sh, uint32_t& cnt, uint32_t& nbits) const {
+    const uint32_t Wp = sh.pre ? 1 : sh.W;
     const uint32_t rbits = opts.bitsum_radix == 8 ? 3u : 1u;
     // a G2 addition costs 1.3 us on a host core against 0.45 us in G1, and the G2 tail is never the last to finish:
     // run it further down on the GPU
     const size_t host_nodes = sizeof(F) > sizeof(Fq) ? HOST_TREE_NODES / 8 : HOST_TREE_NODES;
-    cnt = pl.sh.B; nbits = 0;
+    cnt = sh.B; nbits = 0;
+    if (sh.n == 0) return 0;
     while (cnt >= (1u << rbits) && (size_t)Wp * cnt > host_nodes) { cnt >>= rbits; nbits += rbits; }
-    return (size_t)pl.sh.K * Wp * cnt * (1 + (size_t)nbits);
+    return (size_t)sh.K * Wp * cnt * (1 + (size_t)nbits);
   }
-
+  template <class F>
+  size_t slot_bytes(const MsmShape& sh) const { uint32_t cnt, nbits; return tail_levels<F>(sh, cnt, nbits) * sizeof(XYZZ<F>); }
   // phase 2 (side stream): reduce chunk-boundary partials, then the bucket reduction by bit sums.  Latency-bound
   // (7 dependent point additions per level), so it runs on a high-priority stream underneath the next MSM's accumulation.
   template <class F>
-  void msm_tail(const MsmPlan& pl, MsmWs& ws, XYZZ<F>* win_out /* K * MAXW entries */, StageTimer* tm = nullptr, const char* tail_name = nullptr) {
+  void msm_tail(const MsmPlan& pl, MsmWs& ws, XYZZ<F>* win_out, size_t win_entries, StageTimer* tm = nullptr, const char* tail_name = nullptr) {
     typedef XYZZ<F> X;
     if (pl.sh.n == 0) return;
     Stream ts = tail_stream(ws);
@@ -1330,7 +1366,7 @@ class Engine : public EngineBase {
     }
     const X* inA = buckets; const X* inP = nullptr;
     uint32_t cnt = B, lvl = 0, nbits = 0, end_cnt = 0, end_bits = 0;
-    const size_t out_entries = tail_levels<F>(pl, end_cnt, end_bits);
+    const size_t out_entries = tail_levels<F>(pl.sh, end_cnt, end_bits);
     while (nbits < end_bits) {
       X* oA = (X*)ws.tree[lvl & 1].p; X* oP = (X*)ws.tree[2 + (lvl & 1)].p;
       const X* iA = inA; const X* iP = inP;
@@ -1347,8 +1383,7 @@ class Engine : public EngineBase {
     // result slot: [A : W*cnt][pending 0 : W*cnt] ... [pending nbits-1 : W*cnt]; the host finishes (host_finish)
     ws.tree_cnt = cnt; ws.tree_bits = nbits;
     const size_t nodes = (size_t)W * cnt;
-    ws.out_entries = out_entries;
-    if (ws.out_entries > (size_t)MAXW * pl.sh.K) throw Error(ZKB_E_INTERNAL, "msm result slot overflow");
+    if (out_entries > win_entries) throw Error(ZKB_E_INTERNAL, "msm result slot overflow");
     d2d(ts, win_out, inA, nodes * sizeof(X));
     if (nbits) d2d(ts, win_out + nodes, inP, nodes * nbits * sizeof(X));
     if (tm && tail_name) tm->end_on(ts, span);
@@ -1356,10 +1391,10 @@ class Engine : public EngineBase {
   }
 
   template <class F>
-  void msm_exec(const MsmPlan& pl, const Affine<F>* pts, XYZZ<F>* win_out, MsmWs& ws, StageTimer* tm = nullptr,
+  void msm_exec(const MsmPlan& pl, const Affine<F>* pts, XYZZ<F>* win_out, size_t win_entries, MsmWs& ws, StageTimer* tm = nullptr,
                 const char* accum_name = nullptr, uint32_t view = 0, const char* tail_name = nullptr) {
     msm_accumulate<F>(pl, pts, ws, tm, accum_name, view);
-    msm_tail<F>(pl, ws, win_out, tm, tail_name);
+    msm_tail<F>(pl, ws, win_out, win_entries, tm, tail_name);
   }
 
   // Host finish of one MSM.  Per window: total = sum_k A_k, hi = sum_k k A_k (running sums), S_bit = sum_k P_bit[k];
@@ -1726,13 +1761,61 @@ class Engine : public EngineBase {
 
   // ------------------------------------------------------------------------------ prove
   DevBuf<Fr> scratch_a_, scratch_b_;
-  static constexpr uint32_t MAXW = 1024;  // result slot entries per MSM: (1 + 3 levels) * W * tree_cnt <= 19 * 32
 
   struct HostPartial {  // same layout as Partial
     HG1X h, l, a, b1;
     HG2X b2;
   };
   static_assert(sizeof(HostPartial) == sizeof(Partial), "partial layout");
+
+  // The packed result slots of an MsmSet for K proofs under pk with the z-MSM mode pre_c_z.  The shapes follow from the sizes
+  // and the window widths, so the layout is known before the plans are built (a single proof enqueues its z-MSMs before its h
+  // plan exists).
+  void msm_slots(MsmSet& s, const Pk& pk, uint32_t pre_c_z, uint32_t K) {
+    const MsmShape shz = plan_shape(pk.hi - pk.lo, pre_c_z, K), shh = plan_shape(pk.hhi - pk.hlo, pk.pre_ch, K);
+    const size_t bytes[5] = {slot_bytes<Fq>(shh), slot_bytes<Fq>(shz), slot_bytes<Fq>(shz), slot_bytes<Fq>(shz), slot_bytes<Fq2>(shz)};
+    for (int k = 0; k < 5; k++) s.off[k + 1] = s.off[k] + bytes[k];
+    s.d_win.ensure(s.off[5]);
+    s.hw.ensure(s.off[5]);
+  }
+
+  // MSM k of a set (points pts, the plan's view `view`) into its result slot.  Stage names: [batch][slot][accumulate, tail].
+  static constexpr const char* MSM_STAGES[2][5][2] = {
+      {{"accum1_g1_h", "tail_g1_h"}, {"accum1_g1_l", "tail_g1_l"}, {"accum1_g1_a", "tail_g1_a"}, {"accum1_g1_b1", "tail_g1_b1"},
+       {"accum1_g2_b2", "tail_g2_b2"}},
+      {{"accum1_g1_h_batch", "tail_g1_h_batch"}, {"accum1_g1_l_batch", "tail_g1_l_batch"}, {"accum1_g1_a_batch", "tail_g1_a_batch"},
+       {"accum1_g1_b1_batch", "tail_g1_b1_batch"}, {"accum1_g2_b2_batch", "tail_g2_b2_batch"}}};
+  template <class F>
+  void msm_set_exec(MsmSet& s, int k, const Affine<F>* pts, uint32_t view, StageTimer& tm, bool batch) {
+    const char* const* names = MSM_STAGES[batch][k];
+    msm_exec<F>(s.plan(k), pts, (XYZZ<F>*)(s.d_win.p + s.off[k]), (s.off[k + 1] - s.off[k]) / sizeof(XYZZ<F>), s.ws[k], &tm, names[0],
+                view, names[1]);
+  }
+  // the four MSMs over z, G2 first: b2, l, a, b1 (views 2, 0, 1, 2)
+  void msm_set_z(MsmSet& s, const Pk& pk, StageTimer& tm, bool batch) {
+    msm_set_exec<Fq2>(s, 4, pk.b2.p, 2, tm, batch);
+    msm_set_exec<Fq>(s, 1, pk.l.p, 0, tm, batch);
+    msm_set_exec<Fq>(s, 2, pk.a.p, 1, tm, batch);
+    msm_set_exec<Fq>(s, 3, pk.b1.p, 2, tm, batch);
+  }
+  void msm_set_h(MsmSet& s, const Pk& pk, StageTimer& tm, bool batch) { msm_set_exec<Fq>(s, 0, pk.h.p, 0, tm, batch); }
+
+  // Proof k's five partial sums from the set's result slots on the host (a few hundred point additions each).  `policy`
+  // std::launch::async runs the five on their own host threads, std::launch::deferred on the caller's.
+  HostPartial host_partial(const MsmSet& s, uint32_t k, std::launch policy) const {
+    auto g1 = [&s, k](int slot) {
+      const MsmPlan& pl = s.plan(slot);
+      return pl.sh.n ? host_finish<HG1X>((const HG1X*)(s.hw.p + s.off[slot]), pl, s.ws[slot], k) : HG1X::identity();
+    };
+    auto f_b2 = std::async(policy, [&s, k] {
+      return s.plan_z.sh.n ? host_finish<HG2X>((const HG2X*)(s.hw.p + s.off[4]), s.plan_z, s.ws[4], k) : HG2X::identity();
+    });
+    auto f_h = std::async(policy, g1, 0), f_l = std::async(policy, g1, 1), f_a = std::async(policy, g1, 2);
+    HostPartial hp;
+    hp.b1 = g1(3);
+    hp.h = f_h.get(); hp.l = f_l.get(); hp.a = f_a.get(); hp.b2 = f_b2.get();
+    return hp;
+  }
 
   // sample the assignment: a witness dominated by 0/1 values (hash circuits) makes the z MSMs nearly free, and the
   // proof time is then set by the reduction tails — the windows mode (16 x 2^15 buckets) has the shallower reduction.
@@ -1743,7 +1826,12 @@ class Engine : public EngineBase {
     return cnt && small * 2 > cnt;
   }
 
-  bool z_window_mode(bool sparse) const { return opts.z_mode == 2 || (opts.z_mode == 0 && sparse); }
+  // The z-MSM mode of a proof or a batch from a sample of its assignments, `sparse` of `sampled` of them sparse: the window
+  // tables (pk.pre_cz, one shared bucket set), or 0 for the per-window bucket sets.  ZKB_OPT_Z_MODE: 0 by the sample, 1 tables, 2 windows.
+  uint32_t z_pre_c(const Pk& pk, uint32_t sparse, uint32_t sampled) const {
+    const bool windows = opts.z_mode == 2 || (opts.z_mode == 0 && 2 * sparse > sampled);
+    return windows ? 0 : pk.pre_cz;
+  }
 
   // One proof's device work is ENQUEUED in two steps and COLLECTED in a third, so that (a) the host can exchange witness-map
   // chains between the ranks in the middle and (b) two proofs can be in flight (ProofSlot):
@@ -1793,13 +1881,6 @@ class Engine : public EngineBase {
       sl.z_src = r.z_canon.p;
       sl.sparse_z = r.sparse_z;
     }
-    const size_t slot1 = MAXW * sizeof(G1X), slot2 = MAXW * sizeof(G2X);
-    sl.d_win.ensure(4 * slot1 + slot2);
-    sl.hw.ensure(4 * slot1 + slot2);
-    G1X* w_l = (G1X*)(sl.d_win.p + slot1);
-    G1X* w_a = (G1X*)(sl.d_win.p + 2 * slot1);
-    G1X* w_b1 = (G1X*)(sl.d_win.p + 3 * slot1);
-    G2X* w_b2 = (G2X*)(sl.d_win.p + 4 * slot1);
     // The witness map (3 SpMV, 7 NTT, latency/bandwidth-bound at this size) and the h digit plan go to a second
     // (high-priority) stream and fill the multiply-pipe bubbles of the z-dependent MSMs running on the main stream.
     if (!has_wm_stream_) { wm_stream_ = stream_create_high_priority(); has_wm_stream_ = true; }
@@ -1809,26 +1890,27 @@ class Engine : public EngineBase {
     // flight it overlaps the PREVIOUS proof's accumulate kernels (memory- and atomic-bound work under multiply-bound work)
     // instead of heading the main stream.  Measured: no gain (17.47 vs 17.46 ms per proof) — the GPU is work-bound and the
     // overlapped plan slows the accumulate kernels by what it saves; kept as an option, off by default.
-    const uint32_t pre_c_z = z_window_mode(sl.sparse_z) ? 0 : pk.pre_cz;
+    const uint32_t pre_c_z = z_pre_c(pk, sl.sparse_z ? 1 : 0, 1);
+    msm_slots(sl.msm, pk, pre_c_z, 1);
     if (opts.plan_stream) {
       if (!has_plan_stream_) { plan_stream_ = stream_create_high_priority(); has_plan_stream_ = true; }
       const size_t span = tm.begin_on(plan_stream_, "msm_plan_z");
       StreamScope sc(st_, plan_stream_);
       sl.ev_z_ready.wait(st_);
-      plan_build(sl.plan_z, sl.z_src + 1 + pk.lo, pk.hi - pk.lo, 3, pk.skip.p, pre_c_z);
+      plan_build(sl.msm.plan_z, sl.z_src + 1 + pk.lo, pk.hi - pk.lo, 3, pk.skip.p, pre_c_z);
       tm.end_on(plan_stream_, span);
       sl.ev_plan_z.record(st_);
     }
     if (chain_mask == 7) {   // replicated witness map: underneath the z-dependent MSMs
       StreamScope sc(st_, wm_stream_);
       sl.ev_z_ready.wait(st_);
-      wm_chains(r, sl, chain_mask, *sl.tm2);
+      slot_chains(r, sl, chain_mask, *sl.tm2);
       sl.ev_chains_done.record(st_);
     } else {
       // shared witness map: the other ranks wait for this rank's chains, so they run FIRST and alone on the main stream
       // (0.5 ms with the GPU to themselves; underneath the accumulate kernels they took twice as long and h arrived
       // late: wait_h 1.1 ms at 8 GPUs).  The exchange and the finish step then hide under this rank's z-dependent MSMs.
-      wm_chains(r, sl, chain_mask, tm);
+      slot_chains(r, sl, chain_mask, tm);
       sl.ev_chains_done.record(st_);
     }
     if (opts.plan_stream) {
@@ -1837,13 +1919,10 @@ class Engine : public EngineBase {
       tm.end();
     } else {
       tm.begin("msm_plan_z");
-      plan_build(sl.plan_z, sl.z_src + 1 + pk.lo, pk.hi - pk.lo, 3, pk.skip.p, pre_c_z);
+      plan_build(sl.msm.plan_z, sl.z_src + 1 + pk.lo, pk.hi - pk.lo, 3, pk.skip.p, pre_c_z);
       tm.end();
     }
-    msm_exec<Fq2>(sl.plan_z, pk.b2.p, w_b2, sl.ws[4], &tm, "accum1_g2_b2", 2, "tail_g2_b2");
-    msm_exec<Fq>(sl.plan_z, pk.l.p, w_l, sl.ws[1], &tm, "accum1_g1_l", 0, "tail_g1_l");
-    msm_exec<Fq>(sl.plan_z, pk.a.p, w_a, sl.ws[2], &tm, "accum1_g1_a", 1, "tail_g1_a");
-    msm_exec<Fq>(sl.plan_z, pk.b1.p, w_b1, sl.ws[3], &tm, "accum1_g1_b1", 2, "tail_g1_b1");
+    msm_set_z(sl.msm, pk, tm, false);
     sl.pk = pkh; sl.r1cs = rh; sl.ticket = next_ticket_++; sl.state = 1; sl.has_rs = false;
     // chains left to other ranks: the caller exchanges buffers next, so this rank's chains must be complete in memory
     if (chain_mask != 7 && !no_host_sync) sl.ev_chains_done.sync();   // the host exchanges the buffers next: wait for the chains only
@@ -1856,34 +1935,27 @@ class Engine : public EngineBase {
     R1cs& r = get_r1cs(sl.r1cs);
     StageTimer& tm = *sl.tm;
     StageTimer& tm2 = *sl.tm2;
-    const size_t slot1 = MAXW * sizeof(G1X);
-    G1X* w_h = (G1X*)sl.d_win.p;
+    MsmSet& ms = sl.msm;
     {
       StreamScope sc(st_, wm_stream_);
-      wm_finish(r, sl.a.p, sl.b.p, sl.c.p, sl.h.p, 1, tm2, "witness_map_finish");
+      wm_finish(r, sl.v.p, sl.h.p, 1, tm2, "witness_map_finish");
       tm2.begin("msm_plan_h");
-      plan_build(sl.plan_h, sl.h.p + pk.hlo, pk.hhi - pk.hlo, 1, nullptr, pk.pre_ch);
+      plan_build(ms.plan_h, sl.h.p + pk.hlo, pk.hhi - pk.hlo, 1, nullptr, pk.pre_ch);
       tm2.end();
       sl.ev_h_ready.record(st_);
     }
     tm.begin("wait_h");
     sl.ev_h_ready.wait(st_);
     tm.end();
-    msm_exec<Fq>(sl.plan_h, pk.h.p, w_h, sl.ws[0], &tm, "accum1_g1_h", 0, "tail_g1_h");
+    msm_set_h(ms, pk, tm, false);
     // the rest happens OFF the main stream, so the next proof's plan and accumulate kernels follow at once
     Stream fs = fin_stream(sl);
-    sl.ws[0].acc_done.wait(fs);
+    ms.ws[0].acc_done.wait(fs);
     size_t span = tm.begin_on(fs, "tails_wait");
-    for (int k = 0; k < 5; k++) sl.ws[k].tail_done.wait(fs);
+    for (auto& w : ms.ws) w.tail_done.wait(fs);
     tm.end_on(fs, span);
     span = tm.begin_on(fs, "d2h_windows");
-    {  // only the entries each tail produced (tree_cnt block totals + the pending bit-sum arrays)
-      const size_t offs[5] = {0, slot1, 2 * slot1, 3 * slot1, 4 * slot1};
-      const size_t esz[5] = {sizeof(G1X), sizeof(G1X), sizeof(G1X), sizeof(G1X), sizeof(G2X)};
-      const MsmPlan* pls[5] = {&sl.plan_h, &sl.plan_z, &sl.plan_z, &sl.plan_z, &sl.plan_z};
-      for (int k = 0; k < 5; k++)
-        if (pls[k]->sh.n) d2h(fs, sl.hw.p + offs[k], sl.d_win.p + offs[k], sl.ws[k].out_entries * esz[k]);
-    }
+    d2h(fs, ms.hw.p, ms.d_win.p, ms.off[5]);
     tm.end_on(fs, span);
     sl.done.record(fs);
     sl.state = 2;
@@ -1891,7 +1963,6 @@ class Engine : public EngineBase {
 
   void slot_collect(ProofSlot& sl, uint8_t* partial_out) {
     if (sl.state != 2) throw Error(ZKB_E_ARG, "proof is not fully enqueued (zkb_groth16_prove_end first)");
-    const size_t slot1 = MAXW * sizeof(G1X);
     try {
       sl.done.sync();             // everything this proof enqueued on any stream precedes `done`
       sl.tm->collect(timings);
@@ -1902,21 +1973,8 @@ class Engine : public EngineBase {
       sl.state = 0;
       throw;
     }
-    HostPartial hp;
-    const uint8_t* hw = sl.hw.p;
     const auto t_host0 = std::chrono::steady_clock::now();
-    // five independent host reductions (a few hundred point additions each): one thread per MSM
-    auto hor1 = [&](size_t k, const MsmPlan& pl) {
-      return pl.sh.n ? host_finish<HG1X>((const HG1X*)(hw + k * slot1), pl, sl.ws[k]) : HG1X::identity();
-    };
-    auto f_b2 = std::async(std::launch::async, [&] {
-      return sl.plan_z.sh.n ? host_finish<HG2X>((const HG2X*)(hw + 4 * slot1), sl.plan_z, sl.ws[4]) : HG2X::identity();
-    });
-    auto f_h = std::async(std::launch::async, [&] { return hor1(0, sl.plan_h); });
-    auto f_l = std::async(std::launch::async, [&] { return hor1(1, sl.plan_z); });
-    auto f_a = std::async(std::launch::async, [&] { return hor1(2, sl.plan_z); });
-    hp.b1 = hor1(3, sl.plan_z);
-    hp.h = f_h.get(); hp.l = f_l.get(); hp.a = f_a.get(); hp.b2 = f_b2.get();
+    const HostPartial hp = host_partial(sl.msm, 0, std::launch::async);   // five independent reductions: one thread per MSM
     timings.push_back({"host_tree_finish", std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_host0).count()});
     memcpy(partial_out, &hp, sizeof hp);
     sl.state = 0;
@@ -1926,11 +1984,7 @@ class Engine : public EngineBase {
   void prove_begin(uint64_t pkh, uint64_t rh, const uint64_t* z, uint32_t chain_mask, void* chain_ptrs[3],
                    uint64_t* chain_bytes) override {
     if (open_ticket_) throw Error(ZKB_E_ARG, "a proof is already open on this context (call zkb_groth16_prove_end)");
-    const uint64_t t = slot_begin(pkh, rh, z, chain_mask);
-    open_ticket_ = t;
-    ProofSlot& sl = slot_of(t);
-    if (chain_ptrs) { chain_ptrs[0] = sl.a.p; chain_ptrs[1] = sl.b.p; chain_ptrs[2] = sl.c.p; }
-    if (chain_bytes) *chain_bytes = ((size_t)1 << get_r1cs(rh).log_n) * FRB;
+    open_ticket_ = prove_begin_async(pkh, rh, z, chain_mask, chain_ptrs, chain_bytes);
   }
   void prove_end(uint64_t pkh, uint64_t rh, uint8_t* partial_out) override {
     if (!open_ticket_) throw Error(ZKB_E_ARG, "zkb_groth16_prove_end without a matching prove_begin");
@@ -1949,9 +2003,9 @@ class Engine : public EngineBase {
   uint64_t prove_begin_async(uint64_t pkh, uint64_t rh, const uint64_t* z, uint32_t chain_mask, void* chain_ptrs[3],
                              uint64_t* chain_bytes) override {
     const uint64_t t = slot_begin(pkh, rh, z, chain_mask);
-    ProofSlot& sl = slot_of(t);
-    if (chain_ptrs) { chain_ptrs[0] = sl.a.p; chain_ptrs[1] = sl.b.p; chain_ptrs[2] = sl.c.p; }
-    if (chain_bytes) *chain_bytes = ((size_t)1 << get_r1cs(rh).log_n) * FRB;
+    const size_t n = (size_t)1 << get_r1cs(rh).log_n;
+    if (chain_ptrs) for (int k = 0; k < 3; k++) chain_ptrs[k] = slot_of(t).v.p + k * n;   // the chains the exchange reads and writes
+    if (chain_bytes) *chain_bytes = n * FRB;
     return t;
   }
   // Stream-ordered chain exchange (no host synchronisation): the caller's stream (NCCL / torch) waits for this rank's chains,
@@ -2129,23 +2183,9 @@ class Engine : public EngineBase {
   // parallel on host threads.
   struct BatchState {
     DevBuf<Fr> zc, zm, v, h;    // assignments (canonical, back to back; Montgomery, interleaved), 3K chains, K h vectors
-    MsmPlan plan_z, plan_h;
-    MsmWs ws[5];                // h, l, a, b1, b2
-    DevBuf<uint8_t> d_win;      // the K x 5 result slots, packed
-    HostBuf hw;
-    void destroy() { for (auto& w : ws) w.destroy(); }
-    size_t device_bytes() const {
-      size_t b = zc.bytes() + zm.bytes() + v.bytes() + h.bytes() + d_win.bytes();
-      for (const MsmPlan* p : {&plan_z, &plan_h})
-        b += p->digits.bytes() + p->ranks.bytes() + p->counts.bytes() + p->offsets.bytes() + p->sorted.bytes() + p->scan_tmp.bytes() +
-             p->view_tile_cnt.bytes() + p->view_tile_off.bytes() + p->view_pre32.bytes() + p->view_mask32.bytes();
-      for (const MsmWs& w : ws) {
-        b += w.buckets.bytes();
-        for (int k = 0; k < 2; k++) b += w.val[k].bytes() + w.key[k].bytes();
-        for (int k = 0; k < 4; k++) b += w.tree[k].bytes();
-      }
-      return b;
-    }
+    MsmSet msm;
+    void destroy() { msm.destroy(); }
+    size_t device_bytes() const { return zc.bytes() + zm.bytes() + v.bytes() + h.bytes() + msm.device_bytes(); }
   } batch_;
   // From this domain size on a batch gains nothing over the two-slot pipeline (which overlaps the witness map with the MSMs
   // and each proof's host tail with the next proof's kernels), so prove_batch drives the slots instead; so it does for a
@@ -2234,9 +2274,10 @@ class Engine : public EngineBase {
       return;
     }
     // one z-MSM mode for the whole batch, from a sample of its assignments
-    uint32_t sampled = 0, sparse = 0;
-    for (uint32_t i = 0; i < std::min(K, 8u); i++, sampled++) sparse += assignment_is_sparse(z + (size_t)i * K / std::min(K, 8u) * zw, rc.m);
-    const uint32_t pre_c_z = z_window_mode(2 * sparse > sampled) ? 0 : pk.pre_cz;
+    const uint32_t ns = std::min(K, 8u);
+    uint32_t sparse = 0;
+    for (uint32_t i = 0; i < ns; i++) sparse += assignment_is_sparse(z + (size_t)i * K / ns * zw, rc.m);
+    const uint32_t pre_c_z = z_pre_c(pk, sparse, ns);
     const uint32_t kp = batch_pass_size(pk, rc, K, pre_c_z);
     std::vector<std::pair<const char*, double>> all, part;
     for (uint32_t k0 = 0; k0 < K; k0 += kp) {
@@ -2252,9 +2293,7 @@ class Engine : public EngineBase {
   void batch_pass(const Pk& pk, R1cs& rc, uint32_t K, const uint64_t* z, const uint64_t* r, const uint64_t* s, uint32_t pre_c_z,
                   uint8_t* proofs_out, std::vector<std::pair<const char*, double>>& times) {
     BatchState& b = batch_;
-    DomainT& d = domain(rc.log_n);
-    const uint32_t lg = rc.log_n;
-    const size_t n = (size_t)1 << lg, m = rc.m;
+    const size_t n = (size_t)1 << rc.log_n, m = rc.m;
     // r * d1, s * d1, rs * d1 and s * d2 need nothing from the GPU: host threads compute them underneath the kernels
     std::vector<FixedMults> fms(K);
     std::future<void> fm_all = std::async(std::launch::async, [&] {
@@ -2271,58 +2310,30 @@ class Engine : public EngineBase {
     {
       const Fr* zc = b.zc.p; Fr* zm = b.zm.p;
       if (z) launch<k_fr_convert>(st_, K * m, ZKB_LAMBDA(size_t t) { zm[(t % m) * K + t / m] = Fr::to_mont(zc[t]); });
-      const uint32_t* rpA = rc.rowptr[0].p; const uint32_t* clA = rc.col[0].p; const Fr* vlA = rc.val[0].p;
-      const uint32_t* rpB = rc.rowptr[1].p; const uint32_t* clB = rc.col[1].p; const Fr* vlB = rc.val[1].p;
-      const uint32_t* rpC = rc.rowptr[2].p; const uint32_t* clC = rc.col[2].p; const Fr* vlC = rc.val[2].p;
-      Fr* v = b.v.p;
-      const uint32_t N = (uint32_t)rc.N, ni = (uint32_t)rc.ni, ngroups = (K + SPMV_GROUP - 1) / SPMV_GROUP;
-      // thread (matrix, group of assignments, row): the row index runs fastest, so the output stores are coalesced
-      launch<k_spmv>(st_, 3 * (size_t)ngroups * n, ZKB_LAMBDA(size_t t) {
-        const uint32_t row = (uint32_t)(t & (n - 1)), q = (uint32_t)(t >> lg), kind = q / ngroups, g = q % ngroups;
-        const uint32_t* rp = kind == 0 ? rpA : kind == 1 ? rpB : rpC;
-        const uint32_t* cl = kind == 0 ? clA : kind == 1 ? clB : clC;
-        const Fr* vl = kind == 0 ? vlA : kind == 1 ? vlB : vlC;
-        spmv_batch_body<Fr, SPMV_GROUP>(rp, cl, vl, zm, K, g * SPMV_GROUP, v + (size_t)kind * K * n, n, N, kind == 0 ? ni : 0, row);
-      });
-      ntt_dif(v, d.tw_inv.p, lg, 3 * K);
-      ntt_dit(v, d.tw_fwd.p, lg, d.cos_fwd.p, 3 * K);   // coset shift fused into the first pass, as in wm_chains
-      wm_finish(rc, v, v + K * n, v + 2 * K * n, b.h.p, K, tm, "witness_map_finish_batch");
+      wm_chains(rc, b.zm.p, K, b.v.p, 0, 3);
+      wm_finish(rc, b.v.p, b.h.p, K, tm, "witness_map_finish_batch");
     }
     tm.end();
+    MsmSet& ms = b.msm;
     tm.begin("msm_plan_z_batch");
-    plan_build(b.plan_z, b.zc.p + 1 + pk.lo, pk.hi - pk.lo, 3, pk.skip.p, pre_c_z, K, m);
+    plan_build(ms.plan_z, b.zc.p + 1 + pk.lo, pk.hi - pk.lo, 3, pk.skip.p, pre_c_z, K, m);
     tm.end();
     tm.begin("msm_plan_h_batch");
-    plan_build(b.plan_h, b.h.p + pk.hlo, pk.hhi - pk.hlo, 1, nullptr, pk.pre_ch, K, n);
+    plan_build(ms.plan_h, b.h.p + pk.hlo, pk.hhi - pk.hlo, 1, nullptr, pk.pre_ch, K, n);
     tm.end();
-    // result slots of the five MSMs (h, l, a, b1: G1; b2: G2), packed so that one copy brings all of them to the host
-    uint32_t tc, tb;
-    const size_t ez = b.plan_z.sh.n ? tail_levels<Fq>(b.plan_z, tc, tb) : 0, ez2 = b.plan_z.sh.n ? tail_levels<Fq2>(b.plan_z, tc, tb) : 0;
-    const size_t eh = b.plan_h.sh.n ? tail_levels<Fq>(b.plan_h, tc, tb) : 0;
-    const size_t off[6] = {0, eh * sizeof(G1X), (eh + ez) * sizeof(G1X), (eh + 2 * ez) * sizeof(G1X), (eh + 3 * ez) * sizeof(G1X),
-                           (eh + 3 * ez) * sizeof(G1X) + ez2 * sizeof(G2X)};
-    b.d_win.ensure(off[5]);
-    b.hw.ensure(off[5]);
-    uint8_t* dw = b.d_win.p;
-    msm_exec<Fq2>(b.plan_z, pk.b2.p, (G2X*)(dw + off[4]), b.ws[4], &tm, "accum1_g2_b2_batch", 2, "tail_g2_b2_batch");
-    msm_exec<Fq>(b.plan_z, pk.l.p, (G1X*)(dw + off[1]), b.ws[1], &tm, "accum1_g1_l_batch", 0, "tail_g1_l_batch");
-    msm_exec<Fq>(b.plan_z, pk.a.p, (G1X*)(dw + off[2]), b.ws[2], &tm, "accum1_g1_a_batch", 1, "tail_g1_a_batch");
-    msm_exec<Fq>(b.plan_z, pk.b1.p, (G1X*)(dw + off[3]), b.ws[3], &tm, "accum1_g1_b1_batch", 2, "tail_g1_b1_batch");
-    msm_exec<Fq>(b.plan_h, pk.h.p, (G1X*)(dw + off[0]), b.ws[0], &tm, "accum1_g1_h_batch", 0, "tail_g1_h_batch");
-    for (auto& w : b.ws) w.tail_done.wait(st_);
+    msm_slots(ms, pk, pre_c_z, K);
+    msm_set_z(ms, pk, tm, true);
+    msm_set_h(ms, pk, tm, true);
+    for (auto& w : ms.ws) w.tail_done.wait(st_);
     tm.begin("d2h_windows_batch");
-    d2h(st_, b.hw.p, dw, off[5]);
+    d2h(st_, ms.hw.p, ms.d_win.p, ms.off[5]);
     tm.end();
     stream_sync(st_);
     tm.collect(times);
     fm_all.get();
     const auto t0 = std::chrono::steady_clock::now();
-    const uint8_t* hw = b.hw.p;
     host_parallel(K, [&](uint32_t k) {
-      HostPartial hp;
-      auto g1 = [&](int slot, const MsmPlan& pl) { return pl.sh.n ? host_finish<HG1X>((const HG1X*)(hw + off[slot]), pl, b.ws[slot], k) : HG1X::identity(); };
-      hp.h = g1(0, b.plan_h); hp.l = g1(1, b.plan_z); hp.a = g1(2, b.plan_z); hp.b1 = g1(3, b.plan_z);
-      hp.b2 = b.plan_z.sh.n ? host_finish<HG2X>((const HG2X*)(hw + off[4]), b.plan_z, b.ws[4], k) : HG2X::identity();
+      const HostPartial hp = host_partial(ms, k, std::launch::deferred);
       finalize_with(pk, fms[k], (const uint8_t*)&hp, 1, (const uint32_t*)(r + 4 * (size_t)k), (const uint32_t*)(s + 4 * (size_t)k),
                     proofs_out + (size_t)k * 8 * FQB);
     });
@@ -2386,7 +2397,7 @@ class Engine : public EngineBase {
       prog_witness_pass(p, ns, sin.data(), flags, sz.data(), sf.data());
       uint32_t sparse = 0;
       for (uint32_t i = 0; i < ns; i++) sparse += assignment_is_sparse(&sz[(size_t)i * me * 4], m);
-      pre_c_z = z_window_mode(2 * sparse > ns) ? 0 : (int)pk.pre_cz;
+      pre_c_z = (int)z_pre_c(pk, sparse, ns);
       kp = batch_pass_size(pk, rc, K, (uint32_t)pre_c_z, extra);
       kp = (uint32_t)std::min<uint64_t>(kp, prog_sweep_max(d));
     }
@@ -2420,7 +2431,7 @@ class Engine : public EngineBase {
           stream_sync(st_);
           sparse += assignment_is_sparse(zs.data(), m);
         }
-        pre_c_z = z_window_mode(2 * sparse > ns) ? 0 : (int)pk.pre_cz;
+        pre_c_z = (int)z_pre_c(pk, sparse, ns);
       }
       batch_pass(pk, rc, cnt, nullptr, r + 4 * (size_t)k0, s + 4 * (size_t)k0, (uint32_t)pre_c_z, proofs_out + k0 * pb, part);
       all_t.insert(all_t.end(), part.begin(), part.end());
@@ -2435,32 +2446,40 @@ class Engine : public EngineBase {
   DevBuf<Fr> msm_scalars_;
   MsmPlan plan_misc_;
 
+  // One MSM to a host point on the standalone plan and workspace: build the plan (`replan` false: reuse the previous call's
+  // plan, over the same scalars), accumulate and reduce, copy the result slot back, finish on the host.  With a timer: the
+  // stages msm_plan, msm_exec and accum1.
+  template <class F, class HX>
+  HX msm_host(const Fr* scalars, const Affine<F>* pts, uint64_t n, bool replan, StageTimer* tm = nullptr) {
+    typedef XYZZ<F> X;
+    if (tm) tm->begin("msm_plan");
+    if (replan) plan_build(plan_misc_, scalars, n);
+    if (tm) { tm->end(); tm->begin("msm_exec"); }
+    const size_t bytes = slot_bytes<F>(plan_misc_.sh);
+    d_win_.ensure(bytes);
+    msm_exec<F>(plan_misc_, pts, (X*)d_win_.p, bytes / sizeof(X), ws_misc_, tm, "accum1");
+    ws_misc_.tail_done.wait(st_);
+    if (tm) tm->end();
+    std::vector<uint8_t> hw(bytes);
+    d2h(st_, hw.data(), d_win_.p, bytes);
+    stream_sync(st_);
+    return n ? host_finish<HX>((const HX*)hw.data(), plan_misc_, ws_misc_) : HX::identity();
+  }
+
   template <class F, class HF>
   void msm_t(const uint8_t* points, const uint64_t* scalars, uint64_t n, uint8_t* out) {
     typedef Affine<F> A;
-    typedef XYZZ<F> X;
     typedef XYZZ<HF> HX;
     typedef Affine<HF> HA;
     StageTimer tm(st_);
     msm_pts_.ensure(n * sizeof(A) + 16);
     msm_scalars_.ensure(n + 1);
-    d_win_.ensure(MAXW * sizeof(X));
     A* pts = (A*)msm_pts_.p;
     h2d(st_, pts, points, n * sizeof(A));
     h2d(st_, msm_scalars_.p, scalars, n * FRB);
     pk_convert<F>(pts, n);
-    tm.begin("msm_plan");
-    plan_build(plan_misc_, msm_scalars_.p, n);
-    tm.end();
-    tm.begin("msm_exec");
-    msm_exec<F>(plan_misc_, pts, (X*)d_win_.p, ws_misc_, &tm, "accum1");
-    ws_misc_.tail_done.wait(st_);
-    tm.end();
-    std::vector<uint8_t> hw(MAXW * sizeof(X));
-    d2h(st_, hw.data(), d_win_.p, ws_misc_.out_entries * sizeof(X));
-    stream_sync(st_);
+    const HX res = msm_host<F, HX>(msm_scalars_.p, pts, n, true, &tm);
     tm.collect(timings);
-    HX res = n ? host_finish<HX>((const HX*)hw.data(), plan_misc_, ws_misc_) : HX::identity();
     HA a = HX::to_affine(res);
     const size_t words = sizeof(A) / 4;
     uint32_t* o = (uint32_t*)out;
@@ -2516,7 +2535,6 @@ class Engine : public EngineBase {
   std::map<uint64_t, std::unique_ptr<Gm17Pk>> gm17_pks_;
   uint64_t gm17_pk_load(const uint8_t* pk, size_t len) override;
   void gm17_pk_free(uint64_t h) override { if (!gm17_pks_.erase(h)) throw Error(ZKB_E_ARG, "unknown gm17 pk handle"); }
-  template <class F, class HX> HX gm17_msm(const Fr* scalars, const Affine<F>* pts, uint64_t n, bool replan);
   void gm17_prove(uint64_t pk, uint64_t r1cs, const uint64_t* z, const uint64_t* d1, const uint64_t* d2, const uint64_t* r,
                   uint8_t* proof_out) override;
   size_t gm17_setup_size(uint64_t rh) override;

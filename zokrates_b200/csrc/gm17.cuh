@@ -68,23 +68,6 @@ uint64_t Engine<C>::gm17_pk_load(const uint8_t* pk, size_t len) {
   return h;
 }
 
-// one MSM on the shared scratch plan: digits/sort (or the plan built by the previous call when `replan` is false), accumulate,
-// reduce, host finish
-template <class C>
-template <class F, class HX>
-HX Engine<C>::gm17_msm(const Fr* scalars, const Affine<F>* pts, uint64_t n, bool replan) {
-  typedef XYZZ<F> X;
-  if (n == 0) return HX::identity();
-  d_win_.ensure(MAXW * sizeof(X));
-  if (replan) plan_build(plan_misc_, scalars, n);
-  msm_exec<F>(plan_misc_, pts, (X*)d_win_.p, ws_misc_);
-  ws_misc_.tail_done.wait(st_);
-  std::vector<uint8_t> hw(MAXW * sizeof(X));
-  d2h(st_, hw.data(), d_win_.p, ws_misc_.out_entries * sizeof(X));
-  stream_sync(st_);
-  return host_finish<HX>((const HX*)hw.data(), plan_misc_, ws_misc_);
-}
-
 template <class C>
 void Engine<C>::gm17_prove(uint64_t pkh, uint64_t rh, const uint64_t* z, const uint64_t* d1p, const uint64_t* d2p, const uint64_t* rp,
                            uint8_t* proof_out) {
@@ -104,23 +87,14 @@ void Engine<C>::gm17_prove(uint64_t pkh, uint64_t rh, const uint64_t* z, const u
   DomainT& d = domain(lg);
   StageTimer tm(st_);
   tm.begin("gm17_witness_map");
-  DevBuf<Fr> full_m(nv), full_c(nv), va(n), vc(n), vq(n), a2(n), hc(n + 1), t0(N ? N : 1), t1(N ? N : 1), t2(N ? N : 1);
+  DevBuf<Fr> full_m(nv), full_c(nv), va(n), vc(n), vq(n), a2(n), hc(n + 1), abc(N ? 3 * N : 1);
   if (z) h2d(st_, full_c.p, z, m * FRB); else d2d(st_, full_c.p, r.z_canon.p, m * FRB);
   convert(full_c.p, full_m.p, 0, m);
-  {  // A z, B z, C z
-    Fr* outs[3] = {t0.p, t1.p, t2.p};
-    const Fr* zm = full_m.p;
-    for (int k = 0; k < 3; k++) {
-      Fr* out = outs[k];
-      const uint32_t* rpk = r.rowptr[k].p; const uint32_t* cl = r.col[k].p; const Fr* vl = r.val[k].p;
-      const uint32_t Nn = (uint32_t)N;
-      launch<k_spmv>(st_, N, ZKB_LAMBDA(size_t t) { spmv_body<Fr>(rpk, cl, vl, zm, out, Nn, (uint32_t)t); });
-    }
-  }
+  for (uint32_t k = 0; k < 3; k++) spmv<1>(r, full_m.p, 1, abc.p, N, k, k + 1);   // A z, B z, C z at 0, N, 2 N: one launch each
   dev_zero(st_, va.p, n * FRB);
   dev_zero(st_, vc.p, n * FRB);
   {
-    const Fr* az = t0.p; const Fr* bz = t1.p; const Fr* cz = t2.p;
+    const Fr* az = abc.p; const Fr* bz = abc.p + N; const Fr* cz = abc.p + 2 * N;
     Fr* pa = va.p; Fr* pc = vc.p; Fr* fm = full_m.p;
     const size_t mm = m, NN = N;
     // rows 2i, 2i+1:  (A + B)^2 = 4 C + x_i,  (A - B)^2 = x_i   with the extra variable x_i = (A - B)^2 at column m + i
@@ -187,11 +161,11 @@ void Engine<C>::gm17_prove(uint64_t pkh, uint64_t rh, const uint64_t* z, const u
   }
   tm.end();
   tm.begin("gm17_msms");
-  const HG1X s_a = gm17_msm<Fq, HG1X>(full_c.p + 1, pk.a.p, nv - 1, true);
-  const HG1X s_c2 = gm17_msm<Fq, HG1X>(full_c.p + 1, pk.c2.p, nv - 1, false);
-  const HG2X s_b = gm17_msm<Fq2, HG2X>(full_c.p + 1, pk.b.p, nv - 1, false);
-  const HG1X s_c1 = gm17_msm<Fq, HG1X>(full_c.p + ni, pk.c1.p, nv - ni, true);
-  const HG1X s_h = gm17_msm<Fq, HG1X>(hc.p, pk.gz.p, n + 1, true);
+  const HG1X s_a = msm_host<Fq, HG1X>(full_c.p + 1, pk.a.p, nv - 1, true);
+  const HG1X s_c2 = msm_host<Fq, HG1X>(full_c.p + 1, pk.c2.p, nv - 1, false);
+  const HG2X s_b = msm_host<Fq2, HG2X>(full_c.p + 1, pk.b.p, nv - 1, false);
+  const HG1X s_c1 = msm_host<Fq, HG1X>(full_c.p + ni, pk.c1.p, nv - ni, true);
+  const HG1X s_h = msm_host<Fq, HG1X>(hc.p, pk.gz.p, n + 1, true);
   tm.end();
   tm.collect(timings);
   // final combination on the host (ark does the same serially):

@@ -257,21 +257,12 @@ ZKB_HDN inline void fr_convert_body(const Fr* in, Fr* out, int dir, size_t n, si
   out[t] = dir ? Fr::from_mont(in[t]) : Fr::to_mont(in[t]);
 }
 
-// CSR sparse matrix-vector product in Montgomery form; rows >= n_rows are left to the caller.
-template <class Fr>
-ZKB_HDN inline void spmv_body(const uint32_t* rowptr, const uint32_t* col, const Fr* val, const Fr* z, Fr* out,
-                              uint32_t n_rows, uint32_t t) {
-  if (t >= n_rows) return;
-  Fr acc = Fr::zero();
-  for (uint32_t k = rowptr[t]; k < rowptr[t + 1]; k++) acc = Fr::add(acc, Fr::mul(val[k], z[col[k]]));
-  out[t] = acc;
-}
-
-// The same product for a batch of K assignments, G of them per thread: one thread reads a CSR row (columns and
-// coefficients) once and accumulates G dot products.  z is INTERLEAVED, z[col * K + k]: the G values a term needs sit in
-// G * 32 consecutive bytes (one or two cache lines) instead of G lines K * m * 32 bytes apart.  Vector k of the output
-// starts at out + k * n (rows 0 .. n - 1 of the domain): rows below n_rows hold the products, the next n_copy rows
-// z[row - n_rows] (the instance variables of the A chain, n_copy = 0 for B and C), the rest zero.
+// CSR sparse matrix-vector product in Montgomery form for a batch of K assignments, G of them per thread: one thread reads a
+// CSR row (columns and coefficients) once and accumulates G dot products (G = 1 for a single assignment).  z is INTERLEAVED,
+// z[col * K + k]: the G values a term needs sit in G * 32 consecutive bytes (one or two cache lines) instead of G lines
+// K * m * 32 bytes apart.  Vector k of the output starts at out + k * n (rows 0 .. n - 1 of the domain): rows below n_rows
+// hold the products, the next n_copy rows z[row - n_rows] (the instance variables of the A chain, n_copy = 0 for B and C),
+// the rest zero.
 template <class Fr, int G>
 ZKB_HDN inline void spmv_batch_body(const uint32_t* rowptr, const uint32_t* col, const Fr* val, const Fr* z, uint32_t K, uint32_t k0,
                                     Fr* out, size_t n, uint32_t n_rows, uint32_t n_copy, uint32_t row) {
