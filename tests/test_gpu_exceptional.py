@@ -180,12 +180,19 @@ def crafted_key(pool, r1, z, seed):
     z[seg] = small(t[seg] % 8 + 1)
     z[0] = fr_array([1])[0]
     ih = np.where((np.arange(n - 1) // 4096) % 2 == 0, (np.arange(n - 1) // 32) % K, rng.integers(0, K, n - 1))
+    return key_bytes(pool, r1, (ia, ib, il, ih)), (ia, ib, il, ih)
+
+
+def key_bytes(pool, r1, idx):
+    """The ark-format key whose a / b (G1 and G2) / h / l query points are the pool points idx = (ia, ib, il, ih)."""
+    ia, ib, il, ih = idx
+    m, ni, n = r1.num_variables, r1.num_instance, r1.domain_size
     P = pool.point
     head = [P(1, ALPHA), P(2, BETA), P(2, GAMMA), P(2, DELTA), struct.pack("<Q", ni)]
     head += [P(1, 13 + i) for i in range(ni)] + [P(1, BETA), P(1, DELTA)]
     body = [struct.pack("<Q", m), pool.points(1, ia), struct.pack("<Q", m), pool.points(1, ib), struct.pack("<Q", m),
             pool.points(2, ib), struct.pack("<Q", n - 1), pool.points(1, ih), struct.pack("<Q", m - ni), pool.points(1, il[ni:])]
-    return b"".join(head + body), (ia, ib, il, ih)
+    return b"".join(head + body)
 
 
 def expected_proof(pool, r1, z, idx, h, r, s):

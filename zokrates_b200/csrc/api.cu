@@ -457,6 +457,16 @@ int32_t zkb_last_timings(zkb_ctx* ctx, double* ms_out, const char** names_out, i
 }
 uint64_t zkb_launch_count(zkb_ctx* ctx) { return ctx ? launch_counter() - ctx->launches0 : 0; }
 
+#if defined(ZKB_EMU)
+// Test build only (not in zkb.h): the order in which the emulation runs threads and blocks, process-wide (rt.cuh).
+int32_t zkb_emu_launch_order(uint32_t mode, uint64_t seed) {
+  if (mode > EMU_ORDER_SEEDED) { g_err = "unknown launch order"; return ZKB_E_ARG; }
+  emu_order().mode = mode;
+  emu_order().seed = seed;
+  return ZKB_OK;
+}
+#endif
+
 int32_t zkb_peak_probe(zkb_ctx* ctx, int32_t kind, uint32_t iters, double* out) {
   return guard(ctx, [&] {
     if (!out) throw Error(ZKB_E_ARG, "null");

@@ -168,26 +168,89 @@ inline uint64_t& launch_counter() {
   static uint64_t c = 0;
   return c;
 }
+// The order in which the emulation runs a launch's threads, and a block kernel's blocks and the threads of each
+// phase.  The device promises no order, so a kernel whose result depends on it is wrong even when ascending order
+// (the default) hides the race.  The other orders make such a race reproducible on a CPU: descending, or a
+// bijection of [0, n) keyed by the seed and the launch number.  Set through zkb_emu_launch_order (api.cu).
+enum { EMU_ORDER_ASCENDING = 0, EMU_ORDER_DESCENDING = 1, EMU_ORDER_SEEDED = 2 };
+struct EmuOrder {
+  uint32_t mode = EMU_ORDER_ASCENDING;
+  uint64_t seed = 0;
+};
+inline EmuOrder& emu_order() {
+  static EmuOrder o;
+  return o;
+}
+inline uint64_t emu_mix(uint64_t x) {  // splitmix64 finaliser
+  x ^= x >> 30; x *= 0xbf58476d1ce4e5b9ull;
+  x ^= x >> 27; x *= 0x94d049bb133111ebull;
+  return x ^ (x >> 31);
+}
+// Visiting order of one loop of n steps: perm(i) is the index run at step i.  The seeded order is a bijection of
+// [0, 2^k) (2^k >= n) made of odd multiplies, additions and xor-shifts mod 2^k, cycle-walked down to [0, n).
+struct EmuPerm {
+  size_t n, mask = 0;
+  uint32_t mode, shift = 0;
+  uint64_t key[3] = {0, 0, 0};
+  EmuPerm(size_t n_, uint64_t salt) : n(n_), mode(emu_order().mode) {
+    if (mode != EMU_ORDER_SEEDED) return;
+    uint32_t k = 0;
+    while (k < 63 && ((size_t)1 << k) < n) k++;
+    mask = ((size_t)1 << k) - 1;
+    shift = (k + 1) / 2;
+    uint64_t h = emu_mix(emu_order().seed ^ emu_mix(salt + 0x9e3779b97f4a7c15ull));
+    for (auto& v : key) v = h = emu_mix(h + 0x9e3779b97f4a7c15ull);
+  }
+  size_t step(size_t x) const {
+    for (uint64_t v : key) {
+      x = (size_t)(x * (v | 1) + (v >> 32)) & mask;
+      if (shift) x ^= x >> shift;
+    }
+    return x;
+  }
+  size_t operator()(size_t i) const {
+    if (mode == EMU_ORDER_ASCENDING) return i;
+    if (mode == EMU_ORDER_DESCENDING) return n - 1 - i;
+    size_t x = step(i);
+    while (x >= n) x = step(x);
+    return x;
+  }
+};
 template <class Tag, int BLOCK = 128, int MINB = 1, class Fn>
 inline void launch(Stream, size_t n, Fn fn) {
-  if (n) launch_counter()++;
-  for (size_t tid = 0; tid < n; tid++) fn(tid);
+  if (!n) return;
+  uint64_t id = ++launch_counter();
+  EmuPerm perm(n, id);
+  for (size_t i = 0; i < n; i++) fn(perm(i));
 }
+// Phases stay in sequence (each stands for a __syncthreads()); blocks, and threads within a phase, are permuted.
 template <class Tag, int BLOCK, class Fn>
 inline void launch_phased(Stream, size_t nblocks, uint32_t nphases, Fn fn) {
-  if (nblocks) launch_counter()++;
-  for (size_t b = 0; b < nblocks; b++)
-    for (uint32_t ph = 0; ph < nphases; ph++)
-      for (uint32_t t = 0; t < (uint32_t)BLOCK; t++) fn((uint32_t)b, t, ph);
+  if (!nblocks) return;
+  uint64_t id = ++launch_counter();
+  EmuPerm bperm(nblocks, id);
+  for (size_t i = 0; i < nblocks; i++) {
+    uint32_t b = (uint32_t)bperm(i);
+    for (uint32_t ph = 0; ph < nphases; ph++) {
+      EmuPerm tperm(BLOCK, emu_mix(id) ^ ((uint64_t)b << 20) ^ ph);
+      for (uint32_t t = 0; t < (uint32_t)BLOCK; t++) fn(b, (uint32_t)tperm(t), ph);
+    }
+  }
 }
 template <class Tag, int BLOCK, int SMEM_BYTES, class Fn>
 inline void launch_block(Stream, size_t nblocks, uint32_t nphases, Fn fn) {
-  if (nblocks) launch_counter()++;
+  if (!nblocks) return;
+  uint64_t id = ++launch_counter();
   void* smem = malloc(SMEM_BYTES);
   if (!smem) throw Error(ZKB_E_OOM, "malloc");
-  for (size_t b = 0; b < nblocks; b++)
-    for (uint32_t ph = 0; ph < nphases; ph++)
-      for (uint32_t t = 0; t < (uint32_t)BLOCK; t++) fn((uint32_t)b, t, ph, smem);
+  EmuPerm bperm(nblocks, id);
+  for (size_t i = 0; i < nblocks; i++) {
+    uint32_t b = (uint32_t)bperm(i);
+    for (uint32_t ph = 0; ph < nphases; ph++) {
+      EmuPerm tperm(BLOCK, emu_mix(id) ^ ((uint64_t)b << 20) ^ ph);
+      for (uint32_t t = 0; t < (uint32_t)BLOCK; t++) fn(b, (uint32_t)tperm(t), ph, smem);
+    }
+  }
   free(smem);
 }
 inline void* dev_alloc(size_t bytes) {
