@@ -96,6 +96,8 @@ int32_t zkb_ctx_create(int32_t curve, int32_t device, zkb_ctx** out) {
     if (device < 0 || device >= n) throw Error(ZKB_E_ARG, "device index out of range");
     ZKB_CUDA(cudaSetDevice(device));
     ZKB_CUDA(cudaStreamCreateWithFlags(&c->st.s, cudaStreamNonBlocking));
+#else
+    c->st = stream_create();   // every context its own main stream, as on the device
 #endif
     c->eng.reset(curve == ZKB_CURVE_BN128       ? make_engine_bn254(c->st)
                  : curve == ZKB_CURVE_BLS12_381 ? make_engine_bls12_381(c->st)
@@ -117,10 +119,14 @@ void zkb_ctx_destroy(zkb_ctx* ctx) {
 #if !defined(ZKB_EMU)
   cudaSetDevice(ctx->device);
   if (ctx->st.s) cudaStreamSynchronize(ctx->st.s);
+#else
+  emu_drain_all();
 #endif
   ctx->eng.reset();
 #if !defined(ZKB_EMU)
   if (ctx->st.s) cudaStreamDestroy(ctx->st.s);
+#else
+  stream_destroy(ctx->st);
 #endif
   delete ctx;
 }
@@ -463,6 +469,47 @@ int32_t zkb_emu_launch_order(uint32_t mode, uint64_t seed) {
   if (mode > EMU_ORDER_SEEDED) { g_err = "unknown launch order"; return ZKB_E_ARG; }
   emu_order().mode = mode;
   emu_order().seed = seed;
+  return ZKB_OK;
+}
+// Test build only: the stream policy (rt.cuh EMU_STREAMS_*: 0 eager, 1 lazy, 2 seeded) and flags (1: poison new device and
+// pinned memory), process-wide.  Drains whatever the previous policy left queued and resets the statistics.
+int32_t zkb_emu_stream_order(uint32_t mode, uint64_t seed, uint32_t flags) {
+  if (mode > EMU_STREAMS_SEEDED || flags > EMU_STREAM_POISON) { g_err = "unknown stream policy"; return ZKB_E_ARG; }
+  try {
+    emu_set_streams(mode, seed, flags);
+  } catch (const std::exception& e) {
+    g_err = e.what();
+    return ZKB_E_INTERNAL;
+  }
+  return ZKB_OK;
+}
+// out[0]: operations run after an operation enqueued later; out[1]: the most operations queued at once (since the policy was set)
+int32_t zkb_emu_stream_stats(uint64_t out[2]) {
+  if (!out) { g_err = "null"; return ZKB_E_ARG; }
+  EmuStreams& E = emu_streams();
+  std::lock_guard<std::recursive_mutex> lock(E.mu);
+  out[0] = E.reordered;
+  out[1] = E.peak;
+  return ZKB_OK;
+}
+// An emulated stream outside any context, standing in for a caller's stream (torch / NCCL) in the stream-ordered chain
+// exchange (zkb_groth16_prove_chains_to_stream / _stream_to_finish); zkb_emu_stream_copy queues a copy on it.
+int32_t zkb_emu_stream_create(void** out) {
+  if (!out) { g_err = "null"; return ZKB_E_ARG; }
+  *out = (void*)(intptr_t)stream_create().s;
+  return ZKB_OK;
+}
+int32_t zkb_emu_stream_destroy(void* h) {
+  Stream s;
+  s.s = (int)(intptr_t)h;
+  stream_destroy(s);
+  return ZKB_OK;
+}
+int32_t zkb_emu_stream_copy(void* h, void* dst, const void* src, uint64_t bytes) {
+  if (!dst || !src) { g_err = "null"; return ZKB_E_ARG; }
+  Stream s;
+  s.s = (int)(intptr_t)h;
+  d2d(s, dst, src, bytes);
   return ZKB_OK;
 }
 #endif

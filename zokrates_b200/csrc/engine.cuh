@@ -173,9 +173,11 @@ inline void exclusive_scan(Stream st, const uint32_t* counts, uint32_t* offsets,
   ZKB_CUDA(cudaGetLastError());
 #else
   (void)tile_tmp;
-  uint32_t base = 0;
-  for (uint32_t i = 0; i < n; i++) { offsets[i] = base; base += counts[i]; }
-  offsets[n] = base;
+  emu_enqueue(st, [=] {   // one operation on the kernel's stream
+    uint32_t base = 0;
+    for (uint32_t i = 0; i < n; i++) { offsets[i] = base; base += counts[i]; }
+    offsets[n] = base;
+  });
 #endif
 }
 
@@ -590,8 +592,17 @@ class Engine : public EngineBase {
     r1cs_.erase(h);
   }
 
+  // The resident assignment is about to be overwritten on the main stream.  An open proof begun without z (slot_begin) reads
+  // it on the witness-map stream, and nothing orders that read before this write until slot_finish makes the main stream
+  // wait for h: the main stream waits for that proof's chains first.  (The plan stream's read is ordered by ev_plan_z.)
+  void order_resident_write(const R1cs& r) {
+    for (auto& sl : slots_)
+      if (sl.state != 0 && sl.z_src == r.z_canon.p) sl.ev_chains_done.wait(st_);
+  }
+
   void set_assignment(uint64_t h, const uint64_t* z) override {
     R1cs& r = get_r1cs(h);
+    order_resident_write(r);
     h2d(st_, r.z_canon.p, z, r.m * FRB);
     stream_sync(st_);
     r.has_z = true;
@@ -759,6 +770,7 @@ class Engine : public EngineBase {
                         const uint32_t* out_var) override {
     R1cs& r = get_r1cs(rh);
     StageTimer tm(st_);
+    order_resident_write(r);
     if (z_io) h2d(st_, r.z_canon.p, z_io, r.m * FRB);
     else if (!r.has_z) throw Error(ZKB_E_ARG, "no resident assignment");
     DevBuf<uint32_t> d_rows, d_out, d_flag(1);
@@ -975,6 +987,7 @@ class Engine : public EngineBase {
     uint32_t first = 0;
     d2h(st_, &first, d_flag.p, 4);
     d2h(st_, z.data(), zc.p, d.m_ext * FRB);
+    order_resident_write(r);
     d2d(st_, r.z_canon.p, zc.p, d.m * FRB);
     stream_sync(st_);
     tm.collect(timings);
@@ -1198,16 +1211,19 @@ class Engine : public EngineBase {
     }
 #else
     (void)ntiles;
-    const uint32_t M = of0[NB];
-    for (uint32_t v = 0; v < nv; v++) {
-      uint32_t* ofv = pl.offsets.p + (size_t)(v + 1) * (NB + 1);
-      uint32_t* out = sov + (size_t)v * total;
-      uint32_t kept = 0, b = 0;
-      for (uint32_t p = 0; p <= M; p++) {
-        while (b <= NB && of0[b] == p) ofv[b++] = kept;
-        if (p < M && msm_view_keep(sh, skip, so0[p], v + 1)) out[kept++] = so0[p];
+    uint32_t* ofs = pl.offsets.p;
+    emu_enqueue(st_, [=] {   // one operation on the kernel's stream: the list length of0[NB] is read when it runs
+      const uint32_t M = of0[NB];
+      for (uint32_t v = 0; v < nv; v++) {
+        uint32_t* ofv = ofs + (size_t)(v + 1) * (NB + 1);
+        uint32_t* out = sov + (size_t)v * total;
+        uint32_t kept = 0, b = 0;
+        for (uint32_t p = 0; p <= M; p++) {
+          while (b <= NB && of0[b] == p) ofv[b++] = kept;
+          if (p < M && msm_view_keep(sh, skip, so0[p], v + 1)) out[kept++] = so0[p];
+        }
       }
-    }
+    });
 #endif
   }
 
@@ -1283,7 +1299,7 @@ class Engine : public EngineBase {
       {  // the same passes as the device kernel, block after block
         const size_t blocks = (size_t)((out_bound + BA_TILE - 1) / BA_TILE);
         launch_counter()++;
-        for (size_t blk = 0; blk < blocks; blk++) ba_block_emulate<F>(NB, off_in, off_out, srt, pin, out, (uint32_t)blk);
+        emu_enqueue(st_, [=] { for (size_t blk = 0; blk < blocks; blk++) ba_block_emulate<F>(NB, off_in, off_out, srt, pin, out, (uint32_t)blk); });
       }
 #endif
       of = off_out; so = nullptr; cur_pts = out; bound = out_bound;
@@ -2016,7 +2032,9 @@ class Engine : public EngineBase {
     Stream ext; ext.s = (cudaStream_t)ext_stream;
     sl.ev_chains_done.wait(ext);
 #else
-    (void)ticket; (void)ext_stream;
+    ProofSlot& sl = slot_of(ticket);
+    Stream ext; ext.s = (int)(intptr_t)ext_stream;   // an emulated stream (zkb_emu_stream_create)
+    sl.ev_chains_done.wait(ext);
 #endif
   }
   void prove_stream_to_finish(uint64_t ticket, void* ext_stream) override {
@@ -2027,7 +2045,11 @@ class Engine : public EngineBase {
     sl.ev_exchange.record(ext);
     sl.ev_exchange.wait(wm_stream_);
 #else
-    (void)ticket; (void)ext_stream;
+    ProofSlot& sl = slot_of(ticket);
+    Stream ext; ext.s = (int)(intptr_t)ext_stream;
+    if (!has_wm_stream_) throw Error(ZKB_E_INTERNAL, "no witness-map stream");
+    sl.ev_exchange.record(ext);
+    sl.ev_exchange.wait(wm_stream_);
 #endif
   }
   void prove_end_async(uint64_t ticket) override {

@@ -17,6 +17,14 @@
 
 #if !defined(ZKB_EMU)
 #include <cuda_runtime.h>
+#else
+#include <deque>
+#include <functional>
+#include <map>
+#include <memory>
+#include <mutex>
+#include <set>
+#include <vector>
 #endif
 
 namespace zkb {
@@ -161,7 +169,7 @@ inline void host_free_pinned(void* p) { if (p) cudaFreeHost(p); }
 #else  // ------------------------------------------------------------------ host emulation (tests)
 
 struct Stream {
-  int s = 0;
+  int s = 0;   // emulated stream id (stream_create); 0 is a stream like any other
 };
 #define ZKB_LAMBDA [=]
 inline uint64_t& launch_counter() {
@@ -192,13 +200,14 @@ struct EmuPerm {
   size_t n, mask = 0;
   uint32_t mode, shift = 0;
   uint64_t key[3] = {0, 0, 0};
-  EmuPerm(size_t n_, uint64_t salt) : n(n_), mode(emu_order().mode) {
+  // `o`: the order in force when the launch was enqueued (a deferred launch runs later, possibly under another order)
+  EmuPerm(size_t n_, uint64_t salt, const EmuOrder& o = emu_order()) : n(n_), mode(o.mode) {
     if (mode != EMU_ORDER_SEEDED) return;
     uint32_t k = 0;
     while (k < 63 && ((size_t)1 << k) < n) k++;
     mask = ((size_t)1 << k) - 1;
     shift = (k + 1) / 2;
-    uint64_t h = emu_mix(emu_order().seed ^ emu_mix(salt + 0x9e3779b97f4a7c15ull));
+    uint64_t h = emu_mix(o.seed ^ emu_mix(salt + 0x9e3779b97f4a7c15ull));
     for (auto& v : key) v = h = emu_mix(h + 0x9e3779b97f4a7c15ull);
   }
   size_t step(size_t x) const {
@@ -216,70 +225,292 @@ struct EmuPerm {
     return x;
   }
 };
+// ---- emulated streams ---------------------------------------------------------------------------------------------------
+// The device runs a stream's work in order and the streams of a context concurrently, ordered only by events; the host reads
+// a result once a sync says it is there.  Under the default policy (EAGER) every operation runs when it is issued, so a
+// missing Event::wait or sync can never show.  The other policies queue every launch, copy, fill and event per stream
+// (process-wide: all contexts share one device) and run an operation only when the host needs its result:
+//   LAZY    nothing runs until a sync, a copy to pageable memory, a free or a drain; then only the dependency closure of that
+//           point runs (earlier operations of the same stream and, through each event wait, the recording stream up to the
+//           record), the newest ready queue head first.  A reader whose writer nobody waited for runs before it; a writer
+//           that overtakes a reader still queued on another stream runs first.
+//   SEEDED  after every enqueue and in every drain, a seeded random number of ready queue heads runs, picked at random across
+//           streams; a drain finishes its closure in a random interleaving.
+// The calls follow the CUDA semantics the engine relies on: Event::wait binds to the event's last record at call time (a
+// never-recorded event is a no-op); h2d reads a pageable source at call time (CUDA stages it) and a pinned one
+// (host_alloc_pinned) when it runs; d2h to pageable memory returns after the copy, d2h to pinned memory is deferred;
+// dev_free and host_free_pinned drain everything (cudaFree / cudaFreeHost synchronise); dev_alloc is no barrier and, under
+// EMU_STREAM_POISON, returns memory filled with a nonzero pattern (cudaMalloc memory is not zero; a large malloc is).
+// Set through zkb_emu_stream_order (api.cu).
+enum { EMU_STREAMS_EAGER = 0, EMU_STREAMS_LAZY = 1, EMU_STREAMS_SEEDED = 2 };
+enum { EMU_STREAM_POISON = 1u };
+struct EmuOp {
+  uint64_t seq;                 // enqueue number (process-wide)
+  std::function<void()> fn;     // empty: an event record or an event wait
+  int dep_stream = -1;          // an event wait: runs once stream dep_stream has run everything up to dep_seq
+  uint64_t dep_seq = 0;
+};
+struct EmuStreams {
+  std::recursive_mutex mu;
+  uint32_t mode = EMU_STREAMS_EAGER, flags = 0;
+  uint64_t rng = 0, seq = 0;
+  uint64_t max_run = 0;                   // highest enqueue number run so far
+  uint64_t reordered = 0, queued = 0, peak = 0;
+  int next_id = 1;
+  std::map<int, std::deque<EmuOp>> q;
+  std::set<int> dead;                     // destroyed streams whose queue still holds work
+  std::map<uintptr_t, size_t> pinned;     // host_alloc_pinned ranges: base -> bytes
+};
+inline EmuStreams& emu_streams() {
+  static EmuStreams e;
+  return e;
+}
+inline bool emu_eager() { return emu_streams().mode == EMU_STREAMS_EAGER; }
+inline uint64_t emu_rand(EmuStreams& E) { return emu_mix(E.rng += 0x9e3779b97f4a7c15ull); }
+// stream `sid` has run everything up to enqueue number `seq`
+inline bool emu_done(EmuStreams& E, int sid, uint64_t seq) {
+  auto it = E.q.find(sid);
+  return it == E.q.end() || it->second.empty() || it->second.front().seq > seq;
+}
+inline bool emu_ready(EmuStreams& E, const EmuOp& op) { return op.dep_stream < 0 || emu_done(E, op.dep_stream, op.dep_seq); }
+inline void emu_run_head(EmuStreams& E, int sid) {
+  auto it = E.q.find(sid);
+  EmuOp op = std::move(it->second.front());
+  it->second.pop_front();
+  if (it->second.empty() && E.dead.count(sid)) { E.q.erase(it); E.dead.erase(sid); }
+  E.queued--;
+  if (op.seq < E.max_run) E.reordered++;
+  else E.max_run = op.seq;
+  if (op.fn) op.fn();
+}
+// one of the ready heads among `cand`: the newest (LAZY: the order furthest from the issue order), or a random one (SEEDED)
+inline int emu_pick(EmuStreams& E, const std::vector<int>& cand) {
+  if (E.mode == EMU_STREAMS_SEEDED) return cand[emu_rand(E) % cand.size()];
+  int best = cand[0];
+  for (int s : cand) if (E.q[s].front().seq > E.q[best].front().seq) best = s;
+  return best;
+}
+inline void emu_run_random(EmuStreams& E, uint64_t count) {
+  for (uint64_t k = 0; k < count; k++) {
+    std::vector<int> cand;
+    for (auto& kv : E.q) if (!kv.second.empty() && emu_ready(E, kv.second.front())) cand.push_back(kv.first);
+    if (cand.empty()) return;
+    emu_run_head(E, emu_pick(E, cand));
+  }
+}
+// run the dependency closure of (stream sid, enqueue number seq)
+inline void emu_drain(int sid, uint64_t seq) {
+  EmuStreams& E = emu_streams();
+  std::lock_guard<std::recursive_mutex> lock(E.mu);
+  // need[s]: stream s must run everything up to need[s]; grown through every wait in range until nothing changes
+  std::map<int, uint64_t> need{{sid, seq}};
+  for (bool grew = true; grew;) {
+    grew = false;
+    for (auto kv : std::map<int, uint64_t>(need)) {
+      auto q = E.q.find(kv.first);
+      if (q == E.q.end()) continue;
+      for (const EmuOp& op : q->second) {
+        if (op.seq > kv.second) break;
+        if (op.dep_stream < 0) continue;
+        auto it = need.find(op.dep_stream);
+        if (it == need.end() || it->second < op.dep_seq) { need[op.dep_stream] = op.dep_seq; grew = true; }
+      }
+    }
+  }
+  while (!emu_done(E, sid, seq)) {
+    std::vector<int> cand;
+    for (auto& kv : need)
+      if (!emu_done(E, kv.first, kv.second) && emu_ready(E, E.q[kv.first].front())) cand.push_back(kv.first);
+    if (cand.empty()) throw Error(ZKB_E_INTERNAL, "emulated streams: a wait that can never be satisfied");
+    emu_run_head(E, emu_pick(E, cand));
+  }
+}
+inline void emu_drain_all() {
+  EmuStreams& E = emu_streams();
+  std::lock_guard<std::recursive_mutex> lock(E.mu);
+  while (E.queued) {
+    std::vector<int> cand;
+    for (auto& kv : E.q) if (!kv.second.empty() && emu_ready(E, kv.second.front())) cand.push_back(kv.first);
+    if (cand.empty()) throw Error(ZKB_E_INTERNAL, "emulated streams: a wait that can never be satisfied");
+    emu_run_head(E, emu_pick(E, cand));
+  }
+}
+// queue one operation on stream sid (EAGER: run it now); returns its enqueue number (0 when it ran)
+inline uint64_t emu_push(int sid, std::function<void()> fn, int dep_stream = -1, uint64_t dep_seq = 0) {
+  EmuStreams& E = emu_streams();
+  std::lock_guard<std::recursive_mutex> lock(E.mu);
+  EmuOp op;
+  op.seq = ++E.seq;
+  op.fn = std::move(fn);
+  op.dep_stream = dep_stream;
+  op.dep_seq = dep_seq;
+  const uint64_t s = op.seq;
+  E.q[sid].push_back(std::move(op));
+  if (++E.queued > E.peak) E.peak = E.queued;
+  if (E.mode == EMU_STREAMS_SEEDED) emu_run_random(E, emu_rand(E) % 4);
+  return s;
+}
+template <class Fn>
+inline uint64_t emu_enqueue(Stream st, Fn fn) {
+  if (emu_eager()) { fn(); return 0; }
+  return emu_push(st.s, std::function<void()>(std::move(fn)));
+}
+inline bool emu_is_pinned(const void* p, size_t bytes) {
+  EmuStreams& E = emu_streams();
+  std::lock_guard<std::recursive_mutex> lock(E.mu);
+  auto it = E.pinned.upper_bound((uintptr_t)p);
+  if (it == E.pinned.begin()) return false;
+  --it;
+  return (uintptr_t)p + bytes <= it->first + it->second;
+}
+// the stream policy (EMU_STREAMS_*), its seed and EMU_STREAM_POISON; drains what the previous policy left queued
+inline void emu_set_streams(uint32_t mode, uint64_t seed, uint32_t flags) {
+  emu_drain_all();
+  EmuStreams& E = emu_streams();
+  std::lock_guard<std::recursive_mutex> lock(E.mu);
+  E.mode = mode;
+  E.flags = flags;
+  E.rng = emu_mix(seed ^ 0x5eedull);
+  E.reordered = 0;
+  E.peak = 0;
+}
+
 template <class Tag, int BLOCK = 128, int MINB = 1, class Fn>
-inline void launch(Stream, size_t n, Fn fn) {
+inline void launch(Stream st, size_t n, Fn fn) {
   if (!n) return;
-  uint64_t id = ++launch_counter();
-  EmuPerm perm(n, id);
-  for (size_t i = 0; i < n; i++) fn(perm(i));
+  const uint64_t id = ++launch_counter();
+  const EmuOrder o = emu_order();   // the launch order in force at enqueue time
+  emu_enqueue(st, [=] {
+    EmuPerm perm(n, id, o);
+    for (size_t i = 0; i < n; i++) fn(perm(i));
+  });
 }
 // Phases stay in sequence (each stands for a __syncthreads()); blocks, and threads within a phase, are permuted.
 template <class Tag, int BLOCK, class Fn>
-inline void launch_phased(Stream, size_t nblocks, uint32_t nphases, Fn fn) {
+inline void launch_phased(Stream st, size_t nblocks, uint32_t nphases, Fn fn) {
   if (!nblocks) return;
-  uint64_t id = ++launch_counter();
-  EmuPerm bperm(nblocks, id);
-  for (size_t i = 0; i < nblocks; i++) {
-    uint32_t b = (uint32_t)bperm(i);
-    for (uint32_t ph = 0; ph < nphases; ph++) {
-      EmuPerm tperm(BLOCK, emu_mix(id) ^ ((uint64_t)b << 20) ^ ph);
-      for (uint32_t t = 0; t < (uint32_t)BLOCK; t++) fn(b, (uint32_t)tperm(t), ph);
+  const uint64_t id = ++launch_counter();
+  const EmuOrder o = emu_order();
+  emu_enqueue(st, [=] {
+    EmuPerm bperm(nblocks, id, o);
+    for (size_t i = 0; i < nblocks; i++) {
+      uint32_t b = (uint32_t)bperm(i);
+      for (uint32_t ph = 0; ph < nphases; ph++) {
+        EmuPerm tperm(BLOCK, emu_mix(id) ^ ((uint64_t)b << 20) ^ ph, o);
+        for (uint32_t t = 0; t < (uint32_t)BLOCK; t++) fn(b, (uint32_t)tperm(t), ph);
+      }
     }
-  }
+  });
 }
 template <class Tag, int BLOCK, int SMEM_BYTES, class Fn>
-inline void launch_block(Stream, size_t nblocks, uint32_t nphases, Fn fn) {
+inline void launch_block(Stream st, size_t nblocks, uint32_t nphases, Fn fn) {
   if (!nblocks) return;
-  uint64_t id = ++launch_counter();
-  void* smem = malloc(SMEM_BYTES);
-  if (!smem) throw Error(ZKB_E_OOM, "malloc");
-  EmuPerm bperm(nblocks, id);
-  for (size_t i = 0; i < nblocks; i++) {
-    uint32_t b = (uint32_t)bperm(i);
-    for (uint32_t ph = 0; ph < nphases; ph++) {
-      EmuPerm tperm(BLOCK, emu_mix(id) ^ ((uint64_t)b << 20) ^ ph);
-      for (uint32_t t = 0; t < (uint32_t)BLOCK; t++) fn(b, (uint32_t)tperm(t), ph, smem);
+  const uint64_t id = ++launch_counter();
+  const EmuOrder o = emu_order();
+  emu_enqueue(st, [=] {
+    void* smem = malloc(SMEM_BYTES);
+    if (!smem) throw Error(ZKB_E_OOM, "malloc");
+    EmuPerm bperm(nblocks, id, o);
+    for (size_t i = 0; i < nblocks; i++) {
+      uint32_t b = (uint32_t)bperm(i);
+      for (uint32_t ph = 0; ph < nphases; ph++) {
+        EmuPerm tperm(BLOCK, emu_mix(id) ^ ((uint64_t)b << 20) ^ ph, o);
+        for (uint32_t t = 0; t < (uint32_t)BLOCK; t++) fn(b, (uint32_t)tperm(t), ph, smem);
+      }
     }
-  }
-  free(smem);
+    free(smem);
+  });
 }
 inline void* dev_alloc(size_t bytes) {
-  void* p = malloc(bytes ? bytes : 16);
+  if (bytes == 0) bytes = 16;
+  void* p = malloc(bytes);
   if (!p) throw Error(ZKB_E_OOM, "malloc");
+  if (emu_streams().flags & EMU_STREAM_POISON) memset(p, 0x5a, bytes);
   return p;
 }
-inline void dev_free(void* p) { free(p); }
-inline void h2d(Stream, void* dst, const void* src, size_t bytes) { memcpy(dst, src, bytes); }
-inline void d2h(Stream, void* dst, const void* src, size_t bytes) { memcpy(dst, src, bytes); }
-inline void d2d(Stream, void* dst, const void* src, size_t bytes) { memmove(dst, src, bytes); }
-inline void dev_zero(Stream, void* p, size_t bytes) { memset(p, 0, bytes); }
-inline void dev_fill_ff(Stream, void* p, size_t bytes) { memset(p, 0xff, bytes); }
-inline void stream_sync(Stream) {}
-inline Stream stream_create_high_priority() { return Stream(); }
-inline Stream stream_create() { return Stream(); }
-inline void stream_destroy(Stream) {}
+inline void dev_free(void* p) {
+  if (!p) return;
+  if (!emu_eager()) emu_drain_all();
+  free(p);
+}
+inline void h2d(Stream st, void* dst, const void* src, size_t bytes) {
+  if (!bytes) return;
+  if (emu_eager()) { memcpy(dst, src, bytes); return; }
+  if (emu_is_pinned(src, bytes)) { emu_push(st.s, [=] { memcpy(dst, src, bytes); }); return; }
+  std::shared_ptr<std::vector<uint8_t>> staged(new std::vector<uint8_t>((const uint8_t*)src, (const uint8_t*)src + bytes));
+  emu_push(st.s, [=] { memcpy(dst, staged->data(), bytes); });
+}
+inline void d2h(Stream st, void* dst, const void* src, size_t bytes) {
+  if (!bytes) return;
+  if (emu_eager()) { memcpy(dst, src, bytes); return; }
+  const uint64_t seq = emu_push(st.s, [=] { memcpy(dst, src, bytes); });
+  if (!emu_is_pinned(dst, bytes)) emu_drain(st.s, seq);
+}
+inline void d2d(Stream st, void* dst, const void* src, size_t bytes) {
+  if (bytes) emu_enqueue(st, [=] { memmove(dst, src, bytes); });
+}
+inline void dev_zero(Stream st, void* p, size_t bytes) {
+  if (bytes) emu_enqueue(st, [=] { memset(p, 0, bytes); });
+}
+inline void dev_fill_ff(Stream st, void* p, size_t bytes) {
+  if (bytes) emu_enqueue(st, [=] { memset(p, 0xff, bytes); });
+}
+inline void stream_sync(Stream st) {
+  if (!emu_eager()) emu_drain(st.s, emu_streams().seq);
+}
+inline Stream stream_create() {
+  EmuStreams& E = emu_streams();
+  std::lock_guard<std::recursive_mutex> lock(E.mu);
+  Stream s;
+  s.s = E.next_id++;
+  return s;
+}
+inline Stream stream_create_high_priority() { return stream_create(); }
+// work still queued on a destroyed stream runs later, as on the device
+inline void stream_destroy(Stream s) {
+  EmuStreams& E = emu_streams();
+  std::lock_guard<std::recursive_mutex> lock(E.mu);
+  auto it = E.q.find(s.s);
+  if (it == E.q.end()) return;
+  if (it->second.empty()) E.q.erase(it);
+  else E.dead.insert(s.s);
+}
 struct Event {
-  void record(Stream) {}
-  void wait(Stream) {}
-  void sync() {}
-  void destroy() {}
+  int sid = -1;        // the stream and enqueue number of the last record
+  uint64_t seq = 0;
+  void record(Stream s) {
+    if (emu_eager()) return;
+    sid = s.s;
+    seq = emu_push(s.s, std::function<void()>());
+  }
+  void wait(Stream s) {
+    if (!emu_eager() && sid >= 0) emu_push(s.s, std::function<void()>(), sid, seq);
+  }
+  void sync() {
+    if (!emu_eager() && sid >= 0) emu_drain(sid, seq);
+  }
+  void destroy() { sid = -1; }
 };
 inline void* host_alloc_pinned(size_t bytes) {
-  void* p = malloc(bytes ? bytes : 16);
+  if (bytes == 0) bytes = 16;
+  void* p = malloc(bytes);
   if (!p) throw Error(ZKB_E_OOM, "malloc");
+  if (emu_streams().flags & EMU_STREAM_POISON) memset(p, 0x5a, bytes);
+  EmuStreams& E = emu_streams();
+  std::lock_guard<std::recursive_mutex> lock(E.mu);
+  E.pinned[(uintptr_t)p] = bytes;
   return p;
 }
-inline void host_free_pinned(void* p) { free(p); }
+inline void host_free_pinned(void* p) {
+  if (!p) return;
+  if (!emu_eager()) emu_drain_all();
+  {
+    EmuStreams& E = emu_streams();
+    std::lock_guard<std::recursive_mutex> lock(E.mu);
+    E.pinned.erase((uintptr_t)p);
+  }
+  free(p);
+}
 
 #endif
 
