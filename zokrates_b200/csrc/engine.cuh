@@ -295,6 +295,27 @@ struct FixedBase {
   DevBuf<XYZZ<F>> bases;
 };
 
+// Bounds-checked reads of a proving key in ark's `serialize_unchecked` layout: fixed-size fields, and vectors behind a u64
+// length.  Every overrun and leftover byte is ZKB_E_FORMAT.
+struct KeyReader {
+  const uint8_t* pk;
+  size_t len, off = 0;
+  const uint8_t* take(size_t k) {
+    if (k > len - off) throw Error(ZKB_E_FORMAT, "proving key truncated");
+    off += k;
+    return pk + off - k;
+  }
+  std::pair<const uint8_t*, uint64_t> take_vec(size_t elem) {
+    uint64_t count;
+    memcpy(&count, take(8), 8);
+    if (count > (len - off) / elem) throw Error(ZKB_E_FORMAT, "proving key: vector length");
+    return {take(count * elem), count};
+  }
+  void finish() const {
+    if (off != len) throw Error(ZKB_E_FORMAT, "trailing bytes after proving key");
+  }
+};
+
 template <class FrP, class FqP>
 struct CurveT {
   typedef Fp<FrP> Fr;
@@ -1629,36 +1650,21 @@ class Engine : public EngineBase {
       if (prepared_.fut.valid()) prepared_.fut.wait();
       idle_pk_.reset();
     }
-    size_t off = 0;
-    auto need = [&](size_t k) { if (off + k > len) throw Error(ZKB_E_FORMAT, "proving key truncated"); };
-    auto take = [&](size_t k) { need(k); const uint8_t* p = pk + off; off += k; return p; };
-    auto take_len = [&]() { need(8); uint64_t v; memcpy(&v, pk + off, 8); off += 8; return v; };
-    const uint8_t* alpha1 = take(G1B);
-    const uint8_t* beta2 = take(G2B);
-    take(G2B);  // gamma_g2 (verifier only)
-    const uint8_t* delta2 = take(G2B);
-    uint64_t ni = take_len();
-    if (ni > (len - off) / G1B) throw Error(ZKB_E_FORMAT, "gamma_abc length");
-    take(ni * G1B);
-    const uint8_t* beta1 = take(G1B);
-    const uint8_t* delta1 = take(G1B);
-    uint64_t m = take_len();
-    if (m > (len - off) / G1B) throw Error(ZKB_E_FORMAT, "a_query length");
-    const uint8_t* aq = take(m * G1B);
-    uint64_t m1 = take_len();
-    if (m1 != m) throw Error(ZKB_E_FORMAT, "b_g1_query length differs from a_query");
-    const uint8_t* b1q = take(m * G1B);
-    uint64_t m2 = take_len();
-    if (m2 != m) throw Error(ZKB_E_FORMAT, "b_g2_query length differs from a_query");
-    const uint8_t* b2q = take(m * G2B);
-    uint64_t hl = take_len();
-    if (hl > (len - off) / G1B) throw Error(ZKB_E_FORMAT, "h_query length");
-    const uint8_t* hq = take(hl * G1B);
-    uint64_t ll = take_len();
-    if (ll > (len - off) / G1B) throw Error(ZKB_E_FORMAT, "l_query length");
-    const uint8_t* lq = take(ll * G1B);
-    if (off != len) throw Error(ZKB_E_FORMAT, "trailing bytes after proving key");
-    if (ni < 1 || m < ni || ll != m - ni) throw Error(ZKB_E_FORMAT, "inconsistent query lengths");
+    KeyReader rd{pk, len};
+    const uint8_t* alpha1 = rd.take(G1B);
+    const uint8_t* beta2 = rd.take(G2B);
+    rd.take(G2B);  // gamma_g2 (verifier only)
+    const uint8_t* delta2 = rd.take(G2B);
+    const uint64_t ni = rd.take_vec(G1B).second;  // gamma_abc_g1 (verifier only)
+    const uint8_t* beta1 = rd.take(G1B);
+    const uint8_t* delta1 = rd.take(G1B);
+    const auto [aq, m] = rd.take_vec(G1B);
+    const auto [b1q, m1] = rd.take_vec(G1B);
+    const auto [b2q, m2] = rd.take_vec(G2B);
+    const auto [hq, hl] = rd.take_vec(G1B);
+    const auto [lq, ll] = rd.take_vec(G1B);
+    rd.finish();
+    if (ni < 1 || m < ni || m1 != m || m2 != m || ll != m - ni) throw Error(ZKB_E_FORMAT, "inconsistent query lengths");
 
     std::shared_ptr<Pk> p(new Pk());
     p->fp[0] = fp[0]; p->fp[1] = fp[1];
@@ -2546,6 +2552,36 @@ class Engine : public EngineBase {
     else throw Error(ZKB_E_ARG, "field");
   }
 
+  // ------------------------------------------------------------------------------ setup (see setup.cuh)
+  // One field of a proving key in ark's `serialize_unchecked` layout: fixed-base multiples of the G1 or G2 generator, either
+  // one point (its scalar on the host) or a u64 length and `count` points (their scalars on the device).  Montgomery scalars.
+  struct KeySection {
+    int group;  // 1 or 2
+    bool vec;
+    uint64_t count;
+    Fr scalar;
+    const Fr* scalars;
+  };
+  static KeySection point(int group, const Fr& s) { return {group, false, 1, s, nullptr}; }
+  static KeySection points(int group, const Fr* s, uint64_t count) { return {group, true, count, Fr::zero(), s}; }
+  struct Groth16Scalars {
+    Fr alpha, beta, gamma, delta;
+    const Fr *gamma_abc, *a, *b, *h, *l;
+  };
+  // element k of a trapdoor (canonical, 4 u64 limbs each), Montgomery
+  static Fr trapdoor_fr(const uint64_t* td, int k) { Fr c; memcpy(c.v, td + 4 * k, 32); return Fr::to_mont(c); }
+  // Z(tau) = tau^n - 1 over the domain of size n = 2^lg
+  static Fr vanishing_at(Fr tau, uint32_t lg) { for (uint32_t i = 0; i < lg; i++) tau = Fr::sqr(tau); return Fr::sub(tau, Fr::one()); }
+  DevBuf<Fr> lagrange_at(uint32_t lg, Fr tau, DevBuf<Fr>& pw);
+  DevBuf<Fr> mul_transposed(const R1cs& r, int k, const Fr* w);
+  std::vector<KeySection> groth16_key(const R1cs& r, const Groth16Scalars& s);
+  size_t key_size(const std::vector<KeySection>& key);
+  void write_key(const std::vector<KeySection>& key, const uint64_t* gk, uint8_t* pk_out);
+  template <class F> void fb_build(FixedBase<F>& fb, Affine<F> stdgen, const uint32_t* gk);
+  template <class F> void fb_emit(const FixedBase<F>& fb, const Fr* scalars, size_t count, uint32_t* dst);
+  size_t setup_size(uint64_t rh) override;
+  void setup(uint64_t rh, const uint64_t* trapdoor7, uint8_t* pk_out, size_t cap, size_t* len) override;
+
   // ------------------------------------------------------------------------------ GM17 (see gm17.cuh)
   struct Gm17Pk {
     uint64_t ni = 0, nv = 0, nh = 0;            // instance count (incl. one), SAP variables (incl. one), |g_gamma2_z_t|
@@ -2559,14 +2595,20 @@ class Engine : public EngineBase {
   void gm17_pk_free(uint64_t h) override { if (!gm17_pks_.erase(h)) throw Error(ZKB_E_ARG, "unknown gm17 pk handle"); }
   void gm17_prove(uint64_t pk, uint64_t r1cs, const uint64_t* z, const uint64_t* d1, const uint64_t* d2, const uint64_t* r,
                   uint8_t* proof_out) override;
+  struct Gm17Scalars {
+    Fr alpha, beta, gamma, gz, abgz, g2z2;
+    const Fr *query, *a, *c1, *c2, *gz_t;
+  };
+  // the SAP domain: two rows per R1CS row and per public input, and the constant row
+  static uint32_t gm17_log_n(const R1cs& r) {
+    const uint64_t rows = 2 * r.N + 2 * (r.ni - 1) + 1;
+    uint32_t lg = 0;
+    while (((uint64_t)1 << lg) < rows) lg++;
+    return lg;
+  }
+  std::vector<KeySection> gm17_key(const R1cs& r, const Gm17Scalars& s);
   size_t gm17_setup_size(uint64_t rh) override;
   void gm17_setup(uint64_t rh, const uint64_t* trapdoor6, uint8_t* pk_out, size_t cap, size_t* len) override;
-
-  // ------------------------------------------------------------------------------ setup (see setup.cuh)
-  template <class F> void fb_build(FixedBase<F>& fb, Affine<F> stdgen, const uint32_t* gk);
-  template <class F> void fb_emit(const FixedBase<F>& fb, const Fr* scalars, size_t count, uint32_t* dst);
-  size_t setup_size(uint64_t rh) override;
-  void setup(uint64_t rh, const uint64_t* trapdoor7, uint8_t* pk_out, size_t cap, size_t* len) override;
 
  protected:
   Stream st_;

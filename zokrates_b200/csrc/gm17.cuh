@@ -18,31 +18,23 @@ struct k_gm17_build; struct k_gm17_extra; struct k_gm17_h;
 
 template <class C>
 uint64_t Engine<C>::gm17_pk_load(const uint8_t* pk, size_t len) {
-  size_t off = 0;
-  auto need = [&](size_t k) { if (k > len - off) throw Error(ZKB_E_FORMAT, "gm17 proving key truncated"); };
-  auto take = [&](size_t k) { need(k); const uint8_t* p = pk + off; off += k; return p; };
-  auto take_vec = [&](size_t elem, uint64_t& count) {
-    need(8); memcpy(&count, pk + off, 8); off += 8;
-    if (count > (len - off) / elem) throw Error(ZKB_E_FORMAT, "gm17 proving key: vector length");
-    return take(count * elem);
-  };
-  take(G2B);                     // vk.h_g2            (verifier only)
-  take(G1B);                     // vk.g_alpha_g1
-  take(G2B);                     // vk.h_beta_g2
-  take(G1B);                     // vk.g_gamma_g1
-  take(G2B);                     // vk.h_gamma_g2
-  uint64_t ni, na, nb, nc1, nc2, nh;
-  take_vec(G1B, ni);             // vk.query
-  const uint8_t* aq = take_vec(G1B, na);
-  const uint8_t* bq = take_vec(G2B, nb);
-  const uint8_t* c1q = take_vec(G1B, nc1);
-  const uint8_t* c2q = take_vec(G1B, nc2);
-  const uint8_t* g_gamma_z = take(G1B);
-  const uint8_t* h_gamma_z = take(G2B);
-  const uint8_t* g_ab_gamma_z = take(G1B);
-  const uint8_t* g_gamma2_z2 = take(G1B);
-  const uint8_t* gzq = take_vec(G1B, nh);
-  if (off != len) throw Error(ZKB_E_FORMAT, "trailing bytes after gm17 proving key");
+  KeyReader rd{pk, len};
+  rd.take(G2B);                     // vk.h_g2            (verifier only)
+  rd.take(G1B);                     // vk.g_alpha_g1
+  rd.take(G2B);                     // vk.h_beta_g2
+  rd.take(G1B);                     // vk.g_gamma_g1
+  rd.take(G2B);                     // vk.h_gamma_g2
+  const uint64_t ni = rd.take_vec(G1B).second;   // vk.query
+  const auto [aq, na] = rd.take_vec(G1B);
+  const auto [bq, nb] = rd.take_vec(G2B);
+  const auto [c1q, nc1] = rd.take_vec(G1B);
+  const auto [c2q, nc2] = rd.take_vec(G1B);
+  const uint8_t* g_gamma_z = rd.take(G1B);
+  const uint8_t* h_gamma_z = rd.take(G2B);
+  const uint8_t* g_ab_gamma_z = rd.take(G1B);
+  const uint8_t* g_gamma2_z2 = rd.take(G1B);
+  const auto [gzq, nh] = rd.take_vec(G1B);
+  rd.finish();
   if (ni < 1 || na < ni || nb != na || nc2 != na || nc1 != na - ni || nh < 2) throw Error(ZKB_E_FORMAT, "gm17 proving key: inconsistent query lengths");
   std::unique_ptr<Gm17Pk> p(new Gm17Pk());
   p->ni = ni; p->nv = na; p->nh = nh;
@@ -195,54 +187,42 @@ void Engine<C>::gm17_prove(uint64_t pkh, uint64_t rh, const uint64_t* z, const u
 // c_i = sum_rows 4 u_2r C_r[i] (+ ...), extra variables x_r: c = u_2r + u_2r+1, y_j: c = u_(e+2j-1) + u_(e+2j); then every key element is a
 // fixed-base multiple of g or h (same window tables as the Groth16 setup).  Key bytes: ark's `serialize_unchecked` field order.
 template <class C>
+auto Engine<C>::gm17_key(const R1cs& r, const Gm17Scalars& s) -> std::vector<KeySection> {
+  const uint64_t nv = r.m + r.N + (r.ni - 1), n = (uint64_t)1 << gm17_log_n(r);
+  return {point(2, Fr::one()), point(1, s.alpha), point(2, s.beta),      // vk.h_g2, vk.g_alpha_g1, vk.h_beta_g2
+          point(1, s.gamma), point(2, s.gamma),                          // vk.g_gamma_g1, vk.h_gamma_g2
+          points(1, s.query, r.ni),                                      // vk.query
+          points(1, s.a, nv), points(2, s.a, nv),                        // a_query, b_query
+          points(1, s.c1, nv - r.ni), points(1, s.c2, nv),               // c_query_1, c_query_2
+          point(1, s.gz), point(2, s.gz), point(1, s.abgz), point(1, s.g2z2),   // g_gamma_z, h_gamma_z, g_ab_gamma_z, g_gamma2_z2
+          points(1, s.gz_t, n + 1)};                                     // g_gamma2_z_t
+}
+
+template <class C>
 size_t Engine<C>::gm17_setup_size(uint64_t rh) {
-  R1cs& r = get_r1cs(rh);
-  const uint64_t rows = 2 * r.N + 2 * (r.ni - 1) + 1, nv = r.m + r.N + (r.ni - 1);
-  size_t n = 1;
-  while (n < rows) n <<= 1;
-  return 3 * G2B + 2 * G1B + (8 + r.ni * G1B) + (8 + nv * G1B) + (8 + nv * G2B) + (8 + (nv - r.ni) * G1B) + (8 + nv * G1B) + 3 * G1B + G2B +
-         (8 + (n + 1) * G1B);
+  return key_size(gm17_key(get_r1cs(rh), {}));
 }
 
 template <class C>
 void Engine<C>::gm17_setup(uint64_t rh, const uint64_t* trapdoor6, uint8_t* pk_out, size_t cap, size_t* len) {
-  typedef typename GenOf<C>::T Gen;
   R1cs& r = get_r1cs(rh);
   const uint32_t N = (uint32_t)r.N, ni = (uint32_t)r.ni, m = (uint32_t)r.m;
-  const uint64_t rows = 2 * (uint64_t)N + 2 * (ni - 1) + 1;
-  const uint32_t nv = m + N + (ni - 1);
-  uint32_t lg = 0;
-  while (((uint64_t)1 << lg) < rows) lg++;
+  const uint32_t nv = m + N + (ni - 1), lg = gm17_log_n(r);
   const size_t n = (size_t)1 << lg;
   const size_t total = gm17_setup_size(rh);
   if (cap < total) throw Error(ZKB_E_ARG, "pk_out too small");
-  DomainT& d = domain(lg);
-  Fr td[4];
-  for (int k = 0; k < 4; k++) {
-    Fr c;
-    for (int i = 0; i < 8; i++) c.v[i] = ((const uint32_t*)trapdoor6)[k * 8 + i];
-    td[k] = Fr::to_mont(c);
-  }
-  const Fr alpha = td[0], beta = td[1], gamma = td[2], tau = td[3];
-  Fr tn = tau;
-  for (uint32_t i = 0; i < lg; i++) tn = Fr::sqr(tn);
-  const Fr zt = Fr::sub(tn, Fr::one());
+  const Fr alpha = trapdoor_fr(trapdoor6, 0), beta = trapdoor_fr(trapdoor6, 1), gamma = trapdoor_fr(trapdoor6, 2),
+           tau = trapdoor_fr(trapdoor6, 3);
+  const Fr zt = vanishing_at(tau, lg);
   const Fr ab = Fr::add(alpha, beta), g2 = Fr::sqr(gamma), abg = Fr::mul(ab, gamma), gz = Fr::mul(gamma, zt);
   const Fr g2z = Fr::mul(g2, zt), g2z2x2 = Fr::dbl(g2z);
-  // u = ifft(powers of tau) in natural order; powers up to tau^n scaled by gamma^2 Z for g_gamma2_z_t
-  DevBuf<Fr> pw(n), u(n), pwz(n + 1);
+  // u = Lagrange basis at tau over the SAP domain; powers up to tau^n scaled by gamma^2 Z for g_gamma2_z_t
+  DevBuf<Fr> pw, pwz(n + 1);
+  DevBuf<Fr> u = lagrange_at(lg, tau, pw);
   {
-    Fr one = Fr::one();
-    Fr* pp = pw.p; Fr* pz = pwz.p;
-    launch<k_ntt_table>(st_, n, ZKB_LAMBDA(size_t t) { ntt_powers_body<Fr>(tau, one, pp, (uint32_t)n, (uint32_t)t); });
-    launch<k_ntt_table>(st_, n + 1, ZKB_LAMBDA(size_t t) { ntt_powers_body<Fr>(tau, g2z, pz, (uint32_t)n + 1, (uint32_t)t); });
-    d2d(st_, u.p, pw.p, n * FRB);
-    ntt_dif(u.p, d.tw_inv.p, lg);
-    scratch_a_.ensure(n);
-    Fr* src = u.p; Fr* dst = scratch_a_.p;
-    Fr ninv = d.ninv;
-    launch<k_ntt_brev>(st_, n, ZKB_LAMBDA(size_t t) { dst[bitrev32((uint32_t)t, lg)] = Fr::mul(src[t], ninv); });
-    d2d(st_, u.p, scratch_a_.p, n * FRB);
+    const Fr* pp = pw.p; Fr* pz = pwz.p;
+    const Fr tn = Fr::add(zt, Fr::one());
+    launch<k_setup_scalars>(st_, n + 1, ZKB_LAMBDA(size_t t) { pz[t] = Fr::mul(t < n ? pp[t] : tn, g2z); });
   }
   // per R1CS row: u_2r + u_2r+1, u_2r - u_2r+1, 4 u_2r
   DevBuf<Fr> urow[3];
@@ -255,37 +235,8 @@ void Engine<C>::gm17_setup(uint64_t rh, const uint64_t* trapdoor6, uint8_t* pk_o
       p2[i] = Fr::dbl(Fr::dbl(uu[2 * i]));
     });
   }
-  // transposed products (CSC built on the host, as in the Groth16 setup)
   DevBuf<Fr> abc[3];
-  for (int k = 0; k < 3; k++) {
-    const std::vector<uint32_t>& rp = r.h_rowptr[k];
-    const std::vector<uint32_t>& cl = r.h_col[k];
-    const size_t nnz = cl.size();
-    std::vector<uint32_t> colptr(m + 1, 0), rowidx(nnz), perm(nnz);
-    for (size_t i = 0; i < nnz; i++) colptr[cl[i] + 1]++;
-    for (uint32_t i = 0; i < m; i++) colptr[i + 1] += colptr[i];
-    std::vector<uint32_t> cur(colptr.begin(), colptr.end() - 1);
-    for (uint32_t row = 0; row < N; row++)
-      for (uint32_t e = rp[row]; e < rp[row + 1]; e++) {
-        uint32_t pos = cur[cl[e]]++;
-        rowidx[pos] = row;
-        perm[pos] = e;
-      }
-    DevBuf<uint32_t> d_colptr(m + 1), d_rowidx(nnz ? nnz : 1), d_perm(nnz ? nnz : 1);
-    h2d(st_, d_colptr.p, colptr.data(), (m + 1) * 4);
-    h2d(st_, d_rowidx.p, rowidx.data(), nnz * 4);
-    h2d(st_, d_perm.p, perm.data(), nnz * 4);
-    abc[k].alloc(m);
-    Fr* out = abc[k].p;
-    const uint32_t* cp = d_colptr.p; const uint32_t* ri = d_rowidx.p; const uint32_t* pm = d_perm.p;
-    const Fr* vl = r.val[k].p; const Fr* uu = urow[k].p;
-    launch<k_setup_scalars>(st_, m, ZKB_LAMBDA(size_t t) {
-      Fr acc = Fr::zero();
-      for (uint32_t e = cp[t]; e < cp[t + 1]; e++) acc = Fr::add(acc, Fr::mul(vl[pm[e]], uu[ri[e]]));
-      out[t] = acc;
-    });
-    stream_sync(st_);
-  }
+  for (int k = 0; k < 3; k++) abc[k] = mul_transposed(r, k, urow[k].p);
   // a_i and c_i of every SAP variable
   DevBuf<Fr> va(nv), vc(nv);
   {
@@ -315,7 +266,7 @@ void Engine<C>::gm17_setup(uint64_t rh, const uint64_t* trapdoor6, uint8_t* pk_o
     });
   }
   // scalar vectors of the queries
-  DevBuf<Fr> s_a(nv), s_q(ni), s_c1(nv - ni ? nv - ni : 1), s_c2(nv), ks(9);
+  DevBuf<Fr> s_a(nv), s_q(ni), s_c1(nv - ni ? nv - ni : 1), s_c2(nv);
   {
     const Fr* pa = va.p; const Fr* pc = vc.p;
     Fr* oa = s_a.p; Fr* oq = s_q.p; Fr* o1 = s_c1.p; Fr* o2 = s_c2.p;
@@ -326,44 +277,9 @@ void Engine<C>::gm17_setup(uint64_t rh, const uint64_t* trapdoor6, uint8_t* pk_o
       if (t < ni) oq[t] = Fr::add(Fr::mul(gamma, pc[t]), Fr::mul(ab, pa[t]));
       else o1[t - ni] = mix;
     });
-    Fr hostk[9] = {Fr::one(), alpha, beta, gamma, gz, Fr::mul(abg, zt), Fr::mul(g2z, zt), Fr::zero(), Fr::zero()};
-    h2d(st_, ks.p, hostk, sizeof(hostk));
   }
-  FixedBase<Fq> fb1;
-  FixedBase<Fq2> fb2;
-  DevBuf<uint32_t> gk(16);
-  h2d(st_, gk.p, trapdoor6 + 4 * 4, 64);
-  fb_build<Fq>(fb1, std_g1<Gen, Fq>(), gk.p);
-  fb_build<Fq2>(fb2, std_g2<Gen, Fq2>(), gk.p + 8);
-  DevBuf<uint8_t> out(total);
-  uint8_t* ob = out.p;
-  auto emit = [&](auto& fb, const Fr* scalars, size_t count, size_t byte_off) { fb_emit(fb, scalars, count, (uint32_t*)(ob + byte_off)); };
-  auto put_len = [&](uint64_t v, size_t byte_off) { h2d(st_, ob + byte_off, &v, 8); stream_sync(st_); };
-  size_t off = 0;
-  emit(fb2, ks.p + 0, 1, off); off += G2B;                     // vk.h_g2
-  emit(fb1, ks.p + 1, 1, off); off += G1B;                     // vk.g_alpha_g1
-  emit(fb2, ks.p + 2, 1, off); off += G2B;                     // vk.h_beta_g2
-  emit(fb1, ks.p + 3, 1, off); off += G1B;                     // vk.g_gamma_g1
-  emit(fb2, ks.p + 3, 1, off); off += G2B;                     // vk.h_gamma_g2
-  put_len(ni, off); off += 8;
-  emit(fb1, s_q.p, ni, off); off += (size_t)ni * G1B;          // vk.query
-  put_len(nv, off); off += 8;
-  emit(fb1, s_a.p, nv, off); off += (size_t)nv * G1B;          // a_query
-  put_len(nv, off); off += 8;
-  emit(fb2, s_a.p, nv, off); off += (size_t)nv * G2B;          // b_query
-  put_len(nv - ni, off); off += 8;
-  emit(fb1, s_c1.p, nv - ni, off); off += (size_t)(nv - ni) * G1B;   // c_query_1
-  put_len(nv, off); off += 8;
-  emit(fb1, s_c2.p, nv, off); off += (size_t)nv * G1B;         // c_query_2
-  emit(fb1, ks.p + 4, 1, off); off += G1B;                     // g_gamma_z
-  emit(fb2, ks.p + 4, 1, off); off += G2B;                     // h_gamma_z
-  emit(fb1, ks.p + 5, 1, off); off += G1B;                     // g_ab_gamma_z
-  emit(fb1, ks.p + 6, 1, off); off += G1B;                     // g_gamma2_z2
-  put_len(n + 1, off); off += 8;
-  emit(fb1, pwz.p, n + 1, off); off += (n + 1) * G1B;          // g_gamma2_z_t
-  if (off != total) throw Error(ZKB_E_INTERNAL, "gm17 setup size mismatch");
-  d2h(st_, pk_out, ob, total);
-  stream_sync(st_);
+  write_key(gm17_key(r, {alpha, beta, gamma, gz, Fr::mul(abg, zt), Fr::mul(g2z, zt), s_q.p, s_a.p, s_c1.p, s_c2.p, pwz.p}), trapdoor6 + 4 * 4,
+            pk_out);
   *len = total;
 }
 

@@ -94,91 +94,148 @@ void Engine<C>::fb_emit(const FixedBase<F>& fb, const Fr* scalars, size_t count,
 }
 
 template <class C>
+size_t Engine<C>::key_size(const std::vector<KeySection>& key) {
+  size_t bytes = 0;
+  for (const KeySection& s : key) bytes += (s.vec ? 8 : 0) + s.count * (s.group == 1 ? G1B : G2B);
+  return bytes;
+}
+
+// Every point is a fixed-base multiple of g1 = g1_k * G1std or g2 = g2_k * G2std (gk: g1_k, g2_k, 4 limbs each).  The
+// points go to one device buffer and back in one copy; the length prefixes are written into pk_out on the host.
+template <class C>
+void Engine<C>::write_key(const std::vector<KeySection>& key, const uint64_t* gk, uint8_t* pk_out) {
+  typedef typename GenOf<C>::T Gen;
+  DevBuf<uint32_t> dgk(16);
+  h2d(st_, dgk.p, gk, 64);
+  FixedBase<Fq> fb1;
+  FixedBase<Fq2> fb2;
+  fb_build<Fq>(fb1, std_g1<Gen, Fq>(), dgk.p);
+  fb_build<Fq2>(fb2, std_g2<Gen, Fq2>(), dgk.p + 8);
+  std::vector<Fr> single;
+  for (const KeySection& s : key) if (!s.vec) single.push_back(s.scalar);
+  DevBuf<Fr> ds(single.size());
+  h2d(st_, ds.p, single.data(), single.size() * FRB);
+  const size_t total = key_size(key);
+  DevBuf<uint8_t> out(total);
+  size_t off = 0, j = 0;
+  for (const KeySection& s : key) {
+    if (s.vec) off += 8;
+    uint32_t* dst = (uint32_t*)(out.p + off);
+    const Fr* sc = s.vec ? s.scalars : ds.p + j++;
+    if (s.group == 1) fb_emit(fb1, sc, s.count, dst);
+    else fb_emit(fb2, sc, s.count, dst);
+    off += s.count * (s.group == 1 ? G1B : G2B);
+  }
+  d2h(st_, pk_out, out.p, total);
+  stream_sync(st_);
+  off = 0;
+  for (const KeySection& s : key) {
+    if (s.vec) { memcpy(pk_out + off, &s.count, 8); off += 8; }
+    off += s.count * (s.group == 1 ? G1B : G2B);
+  }
+}
+
+// u_j = L_j(tau) over the domain of size n = 2^lg: ifft(tau^0 .. tau^(n-1)), in natural order, Montgomery.  The powers
+// tau^0 .. tau^(n-1) are left in pw.
+template <class C>
+auto Engine<C>::lagrange_at(uint32_t lg, Fr tau, DevBuf<Fr>& pw) -> DevBuf<Fr> {
+  const size_t n = (size_t)1 << lg;
+  DomainT& d = domain(lg);
+  pw.alloc(n);
+  DevBuf<Fr> u(n);
+  Fr* pp = pw.p; Fr* pu = u.p;
+  const Fr one = Fr::one(), ninv = d.ninv;
+  launch<k_ntt_table>(st_, n, ZKB_LAMBDA(size_t t) { ntt_powers_body<Fr>(tau, one, pp, (uint32_t)n, (uint32_t)t); });
+  d2d(st_, pu, pp, n * FRB);
+  ntt_dif(pu, d.tw_inv.p, lg);
+  // bit-reversal permutation in place, scaled by 1/n: the thread of the lower index of each pair swaps it
+  launch<k_ntt_brev>(st_, n, ZKB_LAMBDA(size_t t) {
+    const uint32_t i = (uint32_t)t, j = bitrev32(i, lg);
+    if (j < i) return;
+    const Fr a = pu[i], b = pu[j];
+    pu[i] = Fr::mul(b, ninv);
+    pu[j] = Fr::mul(a, ninv);
+  });
+  return u;
+}
+
+// out = M_k^T w for matrix k (A, B, C) of the R1CS and a weight per row:  out_i = sum_row M_k[row][i] w_row.  The CSC of M_k
+// is built on the host (integer work only).
+template <class C>
+auto Engine<C>::mul_transposed(const R1cs& r, int k, const Fr* w) -> DevBuf<Fr> {
+  const std::vector<uint32_t>& rp = r.h_rowptr[k];
+  const std::vector<uint32_t>& cl = r.h_col[k];
+  const uint32_t N = (uint32_t)r.N, m = (uint32_t)r.m;
+  const size_t nnz = cl.size();
+  std::vector<uint32_t> colptr(m + 1, 0), rowidx(nnz), perm(nnz);
+  for (size_t i = 0; i < nnz; i++) colptr[cl[i] + 1]++;
+  for (uint32_t i = 0; i < m; i++) colptr[i + 1] += colptr[i];
+  std::vector<uint32_t> cur(colptr.begin(), colptr.end() - 1);
+  for (uint32_t row = 0; row < N; row++)
+    for (uint32_t e = rp[row]; e < rp[row + 1]; e++) {
+      uint32_t pos = cur[cl[e]]++;
+      rowidx[pos] = row;
+      perm[pos] = e;
+    }
+  DevBuf<uint32_t> d_colptr(m + 1), d_rowidx(nnz ? nnz : 1), d_perm(nnz ? nnz : 1);
+  h2d(st_, d_colptr.p, colptr.data(), (m + 1) * 4);
+  h2d(st_, d_rowidx.p, rowidx.data(), nnz * 4);
+  h2d(st_, d_perm.p, perm.data(), nnz * 4);
+  DevBuf<Fr> out(m);
+  Fr* po = out.p;
+  const uint32_t* cp = d_colptr.p; const uint32_t* ri = d_rowidx.p; const uint32_t* pm = d_perm.p;
+  const Fr* vl = r.val[k].p;
+  launch<k_setup_scalars>(st_, m, ZKB_LAMBDA(size_t t) {
+    Fr acc = Fr::zero();
+    for (uint32_t e = cp[t]; e < cp[t + 1]; e++) acc = Fr::add(acc, Fr::mul(vl[pm[e]], w[ri[e]]));
+    po[t] = acc;
+  });
+  stream_sync(st_);  // host vectors and the temporary index buffers go out of scope
+  return out;
+}
+
+template <class C>
+auto Engine<C>::groth16_key(const R1cs& r, const Groth16Scalars& s) -> std::vector<KeySection> {
+  const uint64_t n = (uint64_t)1 << r.log_n;
+  return {point(1, s.alpha), point(2, s.beta), point(2, s.gamma), point(2, s.delta),   // alpha_g1, beta_g2, gamma_g2, delta_g2
+          points(1, s.gamma_abc, r.ni),                                               // gamma_abc_g1
+          point(1, s.beta), point(1, s.delta),                                        // beta_g1, delta_g1
+          points(1, s.a, r.m), points(1, s.b, r.m), points(2, s.b, r.m),              // a_query, b_g1_query, b_g2_query
+          points(1, s.h, n - 1), points(1, s.l, r.m - r.ni)};                         // h_query, l_query
+}
+
+template <class C>
 size_t Engine<C>::setup_size(uint64_t rh) {
-  R1cs& r = get_r1cs(rh);
-  const size_t n = (size_t)1 << r.log_n;
-  return G1B + 3 * G2B + 8 + r.ni * G1B + 2 * G1B + (8 + r.m * G1B) * 2 + 8 + r.m * G2B + 8 + (n - 1) * G1B + 8 +
-         (r.m - r.ni) * G1B;
+  return key_size(groth16_key(get_r1cs(rh), {}));
 }
 
 template <class C>
 void Engine<C>::setup(uint64_t rh, const uint64_t* trapdoor7, uint8_t* pk_out, size_t cap, size_t* len) {
-  typedef typename GenOf<C>::T Gen;
   R1cs& r = get_r1cs(rh);
   const uint32_t lg = r.log_n;
   const size_t n = (size_t)1 << lg;
   const size_t total = setup_size(rh);
   if (cap < total) throw Error(ZKB_E_ARG, "pk_out too small");
   StageTimer tm(st_);
-  DomainT& d = domain(lg);
   const uint32_t N = (uint32_t)r.N, ni = (uint32_t)r.ni, m = (uint32_t)r.m;
 
   // trapdoor scalars (host-side constants; a handful of field operations)
-  Fr td[7];
-  for (int k = 0; k < 7; k++) {
-    Fr c;
-    for (int i = 0; i < 8; i++) c.v[i] = ((const uint32_t*)trapdoor7)[k * 8 + i];
-    td[k] = Fr::to_mont(c);
-  }
-  const Fr alpha = td[0], beta = td[1], gamma = td[2], delta = td[3], tau = td[4];
+  const Fr alpha = trapdoor_fr(trapdoor7, 0), beta = trapdoor_fr(trapdoor7, 1), gamma = trapdoor_fr(trapdoor7, 2),
+           delta = trapdoor_fr(trapdoor7, 3), tau = trapdoor_fr(trapdoor7, 4);
   const Fr ginv = Fr::inv(gamma), dinv = Fr::inv(delta);
-  Fr tn = tau;
-  for (uint32_t i = 0; i < lg; i++) tn = Fr::sqr(tn);
-  const Fr zt = Fr::sub(tn, Fr::one());
-  const Fr hscale = Fr::mul(zt, dinv);
+  const Fr hscale = Fr::mul(vanishing_at(tau, lg), dinv);
 
   tm.begin("setup_scalars");
-  // u = ifft(powers of tau), natural order, Montgomery
-  DevBuf<Fr> pw(n), u(n);
-  {
-    Fr one = Fr::one();
-    Fr* pp = pw.p;
-    launch<k_ntt_table>(st_, n, ZKB_LAMBDA(size_t t) { ntt_powers_body<Fr>(tau, one, pp, (uint32_t)n, (uint32_t)t); });
-    d2d(st_, u.p, pw.p, n * FRB);
-    ntt_dif(u.p, d.tw_inv.p, lg);
-    scratch_a_.ensure(n);
-    Fr* src = u.p; Fr* dst = scratch_a_.p;
-    Fr ninv = d.ninv;
-    launch<k_ntt_brev>(st_, n, ZKB_LAMBDA(size_t t) { dst[bitrev32((uint32_t)t, lg)] = Fr::mul(src[t], ninv); });
-    d2d(st_, u.p, scratch_a_.p, n * FRB);
-  }
-  // transposed products via CSC built on the host (integer work only)
+  DevBuf<Fr> pw;
+  DevBuf<Fr> u = lagrange_at(lg, tau, pw);
   DevBuf<Fr> abc[3];
-  for (int k = 0; k < 3; k++) {
-    const std::vector<uint32_t>& rp = r.h_rowptr[k];
-    const std::vector<uint32_t>& cl = r.h_col[k];
-    const size_t nnz = cl.size();
-    std::vector<uint32_t> colptr(m + 1, 0), rowidx(nnz), perm(nnz);
-    for (size_t i = 0; i < nnz; i++) colptr[cl[i] + 1]++;
-    for (uint32_t i = 0; i < m; i++) colptr[i + 1] += colptr[i];
-    std::vector<uint32_t> cur(colptr.begin(), colptr.end() - 1);
-    for (uint32_t row = 0; row < N; row++)
-      for (uint32_t e = rp[row]; e < rp[row + 1]; e++) {
-        uint32_t pos = cur[cl[e]]++;
-        rowidx[pos] = row;
-        perm[pos] = e;
-      }
-    DevBuf<uint32_t> d_colptr(m + 1), d_rowidx(nnz), d_perm(nnz);
-    h2d(st_, d_colptr.p, colptr.data(), (m + 1) * 4);
-    h2d(st_, d_rowidx.p, rowidx.data(), nnz * 4);
-    h2d(st_, d_perm.p, perm.data(), nnz * 4);
-    abc[k].alloc(m);
-    Fr* out = abc[k].p;
-    const uint32_t* cp = d_colptr.p; const uint32_t* ri = d_rowidx.p; const uint32_t* pm = d_perm.p;
-    const Fr* vl = r.val[k].p; const Fr* uu = u.p;
-    const int add_inst = (k == 0);
-    launch<k_setup_scalars>(st_, m, ZKB_LAMBDA(size_t t) {
-      Fr acc = Fr::zero();
-      for (uint32_t e = cp[t]; e < cp[t + 1]; e++) acc = Fr::add(acc, Fr::mul(vl[pm[e]], uu[ri[e]]));
-      if (add_inst && t < ni) acc = Fr::add(acc, uu[N + t]);
-      out[t] = acc;
-    });
-    stream_sync(st_);  // host vectors and the temporary index buffers go out of scope
-  }
-  // combined scalars: gamma_abc / l, and h
+  for (int k = 0; k < 3; k++) abc[k] = mul_transposed(r, k, u.p);
   DevBuf<Fr> lq(m), hq(n);
   {
-    const Fr* pa = abc[0].p; const Fr* pb = abc[1].p; const Fr* pc = abc[2].p;
+    Fr* pa = abc[0].p; const Fr* pb = abc[1].p; const Fr* pc = abc[2].p; const Fr* uu = u.p;
+    // the instance rows x_i * 1 = x_i that ark appends after the constraints
+    launch<k_setup_scalars>(st_, ni, ZKB_LAMBDA(size_t t) { pa[t] = Fr::add(pa[t], uu[N + t]); });
+    // combined scalars: gamma_abc / l, and h
     Fr* pl = lq.p;
     launch<k_setup_scalars>(st_, m, ZKB_LAMBDA(size_t t) {
       Fr v = Fr::add(Fr::add(Fr::mul(beta, pa[t]), Fr::mul(alpha, pb[t])), pc[t]);
@@ -187,53 +244,11 @@ void Engine<C>::setup(uint64_t rh, const uint64_t* trapdoor7, uint8_t* pk_out, s
     Fr* ph = hq.p; const Fr* pp = pw.p;
     launch<k_setup_scalars>(st_, n, ZKB_LAMBDA(size_t t) { ph[t] = Fr::mul(pp[t], hscale); });
   }
-  // the six key scalars alpha, beta, gamma, delta (G1 and G2 as needed)
-  DevBuf<Fr> ks(4);
-  {
-    Fr hostk[4] = {alpha, beta, gamma, delta};
-    h2d(st_, ks.p, hostk, sizeof(hostk));
-  }
   tm.end();
 
-  // fixed-base tables for g1 = g1_k * G1std and g2 = g2_k * G2std
   tm.begin("setup_fixed_base");
-  FixedBase<Fq> fb1;
-  FixedBase<Fq2> fb2;
-  DevBuf<uint32_t> gk(16);
-  h2d(st_, gk.p, trapdoor7 + 5 * 4, 64);
-  const uint32_t* gkp = gk.p;
-  fb_build<Fq>(fb1, std_g1<Gen, Fq>(), gkp);
-  fb_build<Fq2>(fb2, std_g2<Gen, Fq2>(), gkp + 8);
-
-  DevBuf<uint8_t> out(total);
-  uint8_t* ob = out.p;
-  auto emit = [&](auto& fb, const Fr* scalars, size_t count, size_t byte_off) {
-    fb_emit(fb, scalars, count, (uint32_t*)(ob + byte_off));
-  };
-  auto put_len = [&](uint64_t v, size_t byte_off) { h2d(st_, ob + byte_off, &v, 8); stream_sync(st_); };
-  size_t off = 0;
-  emit(fb1, ks.p + 0, 1, off); off += G1B;            // alpha_g1
-  emit(fb2, ks.p + 1, 1, off); off += G2B;            // beta_g2
-  emit(fb2, ks.p + 2, 1, off); off += G2B;            // gamma_g2
-  emit(fb2, ks.p + 3, 1, off); off += G2B;            // delta_g2
-  put_len(ni, off); off += 8;
-  emit(fb1, lq.p, ni, off); off += (size_t)ni * G1B;  // gamma_abc_g1
-  emit(fb1, ks.p + 1, 1, off); off += G1B;            // beta_g1
-  emit(fb1, ks.p + 3, 1, off); off += G1B;            // delta_g1
-  put_len(m, off); off += 8;
-  emit(fb1, abc[0].p, m, off); off += (size_t)m * G1B;  // a_query
-  put_len(m, off); off += 8;
-  emit(fb1, abc[1].p, m, off); off += (size_t)m * G1B;  // b_g1_query
-  put_len(m, off); off += 8;
-  emit(fb2, abc[1].p, m, off); off += (size_t)m * G2B;  // b_g2_query
-  put_len(n - 1, off); off += 8;
-  emit(fb1, hq.p, n - 1, off); off += (n - 1) * G1B;    // h_query
-  put_len(m - ni, off); off += 8;
-  emit(fb1, lq.p + ni, m - ni, off); off += (size_t)(m - ni) * G1B;  // l_query
-  if (off != total) throw Error(ZKB_E_INTERNAL, "setup size mismatch");
+  write_key(groth16_key(r, {alpha, beta, gamma, delta, lq.p, abc[0].p, abc[1].p, hq.p, lq.p + ni}), trapdoor7 + 5 * 4, pk_out);
   tm.end();
-  d2h(st_, pk_out, ob, total);
-  stream_sync(st_);
   *len = total;
   tm.collect(timings);
 }
