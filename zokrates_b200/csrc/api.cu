@@ -33,16 +33,12 @@ static int32_t guard(zkb_ctx* ctx, Fn fn) {
   try {
     if (!ctx || !ctx->eng) throw Error(ZKB_E_ARG, "null context");
     std::lock_guard<std::recursive_mutex> lock(ctx->mu);
-#if !defined(ZKB_EMU)
-    ZKB_CUDA(cudaSetDevice(ctx->device));
-#endif
+    device_select(ctx->device);
     fn();
     return ZKB_OK;
   } catch (const Error& e) {
     g_err = e.what();
-#if !defined(ZKB_EMU)
-    cudaGetLastError();  // clear a sticky launch-configuration error
-#endif
+    clear_device_error();
     return e.code;
   } catch (const std::bad_alloc&) {
     g_err = "host allocation failed";
@@ -62,18 +58,10 @@ const char* zkb_last_error(void) { return g_err.c_str(); }
 uint32_t zkb_abi_version(void) { return 1; }
 
 int32_t zkb_device_count(void) {
-#if !defined(ZKB_EMU)
-  int n = 0;
-  cudaError_t e = cudaGetDeviceCount(&n);
-  if (e != cudaSuccess) {
-    g_err = std::string("cudaGetDeviceCount: ") + cudaGetErrorString(e);
-    cudaGetLastError();
-    return -1;
-  }
+  const char* why = "";
+  const int n = device_count(&why);
+  if (n < 0) g_err = std::string("cudaGetDeviceCount: ") + why;
   return n;
-#else
-  return 1;
-#endif
 }
 
 int32_t zkb_ctx_create(int32_t curve, int32_t device, zkb_ctx** out) {
@@ -85,20 +73,12 @@ int32_t zkb_ctx_create(int32_t curve, int32_t device, zkb_ctx** out) {
     std::unique_ptr<zkb_ctx> c(new zkb_ctx());
     c->curve = curve;
     c->device = device;
-#if !defined(ZKB_EMU)
-    int n = 0;
-    cudaError_t e = cudaGetDeviceCount(&n);
-    if (e != cudaSuccess || n == 0) {
-      cudaGetLastError();
-      throw Error(ZKB_E_CUDA, std::string("no usable CUDA device (libzkb200 has no CPU fallback): ") +
-                                  (e != cudaSuccess ? cudaGetErrorString(e) : "device count is 0"));
-    }
+    const char* why = "device count is 0";
+    const int n = device_count(&why);
+    if (n <= 0) throw Error(ZKB_E_CUDA, std::string("no usable CUDA device (libzkb200 has no CPU fallback): ") + why);
     if (device < 0 || device >= n) throw Error(ZKB_E_ARG, "device index out of range");
-    ZKB_CUDA(cudaSetDevice(device));
-    ZKB_CUDA(cudaStreamCreateWithFlags(&c->st.s, cudaStreamNonBlocking));
-#else
-    c->st = stream_create();   // every context its own main stream, as on the device
-#endif
+    device_select(device);
+    c->st = stream_create();
     c->eng.reset(curve == ZKB_CURVE_BN128       ? make_engine_bn254(c->st)
                  : curve == ZKB_CURVE_BLS12_381 ? make_engine_bls12_381(c->st)
                                                 : make_engine_bls12_377(c->st));
@@ -116,18 +96,9 @@ int32_t zkb_ctx_create(int32_t curve, int32_t device, zkb_ctx** out) {
 
 void zkb_ctx_destroy(zkb_ctx* ctx) {
   if (!ctx) return;
-#if !defined(ZKB_EMU)
-  cudaSetDevice(ctx->device);
-  if (ctx->st.s) cudaStreamSynchronize(ctx->st.s);
-#else
-  emu_drain_all();
-#endif
+  device_drain(ctx->device, ctx->st);
   ctx->eng.reset();
-#if !defined(ZKB_EMU)
-  if (ctx->st.s) cudaStreamDestroy(ctx->st.s);
-#else
   stream_destroy(ctx->st);
-#endif
   delete ctx;
 }
 
@@ -500,16 +471,12 @@ int32_t zkb_emu_stream_create(void** out) {
   return ZKB_OK;
 }
 int32_t zkb_emu_stream_destroy(void* h) {
-  Stream s;
-  s.s = (int)(intptr_t)h;
-  stream_destroy(s);
+  stream_destroy(stream_from_handle(h));
   return ZKB_OK;
 }
 int32_t zkb_emu_stream_copy(void* h, void* dst, const void* src, uint64_t bytes) {
   if (!dst || !src) { g_err = "null"; return ZKB_E_ARG; }
-  Stream s;
-  s.s = (int)(intptr_t)h;
-  d2d(s, dst, src, bytes);
+  d2d(stream_from_handle(h), dst, src, bytes);
   return ZKB_OK;
 }
 #endif

@@ -37,61 +37,6 @@ struct k_msm_accum2; struct k_msm_bitsum; struct k_pk_convert; struct k_final_a;
 struct k_final_c; struct k_final_d; struct k_point_out; struct k_field_op; struct k_setup_scalars; struct k_fixed_base;
 struct k_to_affine; struct k_copy; struct k_msm_view; struct k_solver_level; struct k_ba_halve; struct k_ba_round; struct k_msm_table; struct k_ntt_dif_tile; struct k_ntt_dit_tile; struct k_witness_level;
 
-// ---------------------------------------------------------------------------------------------
-// stage timer: CUDA events on the engine stream (no-op in the host emulation)
-struct StageTimer {
-#if !defined(ZKB_EMU)
-  struct Ev { const char* name; cudaEvent_t a, b; };
-  std::vector<Ev> evs;
-  std::vector<size_t> open;  // stack of stages begun but not ended (stages may nest)
-  Stream st;
-  explicit StageTimer(Stream s) : st(s) {}
-  void begin(const char* name) {
-    Ev e{name, nullptr, nullptr};
-    ZKB_CUDA(cudaEventCreate(&e.a));
-    ZKB_CUDA(cudaEventCreate(&e.b));
-    ZKB_CUDA(cudaEventRecord(e.a, st.s));
-    open.push_back(evs.size());
-    evs.push_back(e);
-  }
-  void end() {
-    size_t i = open.back();
-    open.pop_back();
-    ZKB_CUDA(cudaEventRecord(evs[i].b, st.s));
-  }
-  // spans on other streams (tails): begin_on returns a handle for end_on
-  size_t begin_on(Stream s, const char* name) {
-    Ev e{name, nullptr, nullptr};
-    ZKB_CUDA(cudaEventCreate(&e.a));
-    ZKB_CUDA(cudaEventCreate(&e.b));
-    ZKB_CUDA(cudaEventRecord(e.a, s.s));
-    evs.push_back(e);
-    return evs.size() - 1;
-  }
-  void end_on(Stream s, size_t i) { ZKB_CUDA(cudaEventRecord(evs[i].b, s.s)); }
-  void collect(std::vector<std::pair<const char*, double>>& out) {
-    out.clear();
-    for (auto& e : evs) {
-      ZKB_CUDA(cudaEventSynchronize(e.b));
-      float ms = 0;
-      ZKB_CUDA(cudaEventElapsedTime(&ms, e.a, e.b));
-      out.push_back({e.name, (double)ms});
-      cudaEventDestroy(e.a);
-      cudaEventDestroy(e.b);
-    }
-    evs.clear();
-  }
-  ~StageTimer() { for (auto& e : evs) { cudaEventDestroy(e.a); cudaEventDestroy(e.b); } }
-#else
-  explicit StageTimer(Stream) {}
-  void begin(const char*) {}
-  void end() {}
-  size_t begin_on(Stream, const char*) { return 0; }
-  void end_on(Stream, size_t) {}
-  void collect(std::vector<std::pair<const char*, double>>& out) { out.clear(); }
-#endif
-};
-
 // exclusive scan of NB counters -> offsets[NB+1]
 #if !defined(ZKB_EMU)
 static __global__ void zkb_scan_kernel(const uint32_t* counts, uint32_t* offsets, uint32_t n) {
@@ -117,8 +62,6 @@ static __global__ void zkb_scan_kernel(const uint32_t* counts, uint32_t* offsets
   }
   if (tid == 1023) offsets[n] = sums[1023];
 }
-#endif
-#if !defined(ZKB_EMU)
 // three-phase scan for large n: per-tile sums, scan of the tile sums (single block), per-tile rescan
 static constexpr int SCAN_BLOCK = 256, SCAN_PER = 8, SCAN_TILE = SCAN_BLOCK * SCAN_PER;
 static __global__ void zkb_scan_tile_sums(const uint32_t* in, uint32_t* tile_sums, uint32_t n) {
@@ -417,17 +360,6 @@ class Engine : public EngineBase {
   uint32_t ntt_tile_min() const { return opts.ntt_tile_min < (int64_t)NTT_TILE_LOG ? NTT_TILE_LOG : (uint32_t)opts.ntt_tile_min; }
   uint32_t ntt_max_s() const { return opts.ntt_max_s < 5 ? 5u : (uint32_t)opts.ntt_max_s; }
   bool ntt_tiled(uint32_t log_n) const { return log_n >= ntt_tile_min(); }
-  int sm_count_ = 0;
-  int sm_count() {
-#if !defined(ZKB_EMU)
-    if (!sm_count_) {
-      int dev = 0;
-      ZKB_CUDA(cudaGetDevice(&dev));
-      ZKB_CUDA(cudaDeviceGetAttribute(&sm_count_, cudaDevAttrMultiProcessorCount, dev));
-    }
-#endif
-    return sm_count_ ? sm_count_ : 1;
-  }
 
   // natural -> bit-reversed.  `count` vectors of 2^log_n elements back to back (a batch of proofs): every launch transforms
   // all of them with the same twiddles, a thread or tile finds its vector from its index.
@@ -440,7 +372,7 @@ class Engine : public EngineBase {
       const Fr* nul = nullptr;
 #if !defined(ZKB_EMU)
       if (opts.ntt_kernel == 2) {           // four-step twiddles, cp.async tile load, padded planes (ntt_tile.cuh)
-        for (uint32_t i = 0; i < np; i++) launch_ntt_tile2<Fr, false>(st_, x, tw, nul, ps[i], tiles, sm_count());
+        for (uint32_t i = 0; i < np; i++) launch_ntt_tile2<Fr, false>(st_, x, tw, nul, ps[i], tiles, device_sm_count());
         return;
       }
 #endif
@@ -475,7 +407,7 @@ class Engine : public EngineBase {
       const size_t tiles = (size_t)count << lg_tpv;
 #if !defined(ZKB_EMU)
       if (opts.ntt_kernel == 2) {
-        for (uint32_t i = np; i-- > 0;) launch_ntt_tile2<Fr, true>(st_, x, tw, (i == np - 1) ? scale : nullptr, ps[i], tiles, sm_count());
+        for (uint32_t i = np; i-- > 0;) launch_ntt_tile2<Fr, true>(st_, x, tw, (i == np - 1) ? scale : nullptr, ps[i], tiles, device_sm_count());
         return;
       }
 #endif
@@ -1074,13 +1006,9 @@ class Engine : public EngineBase {
   uint32_t prog_witness_pass_size(const ProgData& d, uint32_t K) {
     uint64_t kmax = std::min<uint64_t>(K, prog_sweep_max(d));
     if (opts.batch_pass_max > 0) kmax = std::min<uint64_t>(kmax, (uint64_t)opts.batch_pass_max);
-#if !defined(ZKB_EMU)
-    size_t free_b = 0, total_b = 0;
-    ZKB_CUDA(cudaMemGetInfo(&free_b, &total_b));
-    const size_t reserve = (size_t)1 << 30, per = (2 * (size_t)d.m_ext + d.arg_ids.size()) * FRB + 4;
-    const uint64_t fit = free_b > reserve ? (free_b - reserve) / per : 0;
+    const size_t free_b = dev_mem_free(), per = (2 * (size_t)d.m_ext + d.arg_ids.size()) * FRB + 4;
+    const uint64_t fit = free_b > DEV_MEM_RESERVE ? (free_b - DEV_MEM_RESERVE) / per : 0;
     kmax = std::min<uint64_t>(kmax, fit);
-#endif
     if (kmax == 0) throw Error(ZKB_E_OOM, "not even one input set fits in device memory");
     return (uint32_t)kmax;
   }
@@ -1591,13 +1519,8 @@ class Engine : public EngineBase {
     // HBM budget: the tables must leave room for the sort plans (digits + 3 sorted views: 16 B per (pair, window)), the bucket
     // sets and the witness-map vectors of the circuit this key belongs to, plus 1 GiB of slack.
     const size_t need_z = (size_t)Wz * cnt * (3 * G1B + G2B), need_h = (size_t)Wh * hcnt * G1B;
-    const size_t reserve = (size_t)16 * (cnt * (Wz ? Wz : 17) + hcnt * (Wh ? Wh : 17)) + 6 * (p.hl + 1) * FRB + ((size_t)1 << 30);
-#if !defined(ZKB_EMU)
-    size_t free_b = 0, total_b = 0;
-    ZKB_CUDA(cudaMemGetInfo(&free_b, &total_b));
-#else
-    size_t free_b = ~(size_t)0 >> 1;
-#endif
+    const size_t reserve = (size_t)16 * (cnt * (Wz ? Wz : 17) + hcnt * (Wh ? Wh : 17)) + 6 * (p.hl + 1) * FRB + DEV_MEM_RESERVE;
+    const size_t free_b = dev_mem_free();
     size_t avail = free_b > reserve ? free_b - reserve : 0;
     auto fits = [&](size_t need, int& status, const char* what) {
       if (status != TAB_BUILT) return false;
@@ -2033,30 +1956,13 @@ class Engine : public EngineBase {
   // Stream-ordered chain exchange (no host synchronisation): the caller's stream (NCCL / torch) waits for this rank's chains,
   // runs its broadcasts, and the finish step waits for whatever that stream has enqueued by then.
   void prove_chains_to_stream(uint64_t ticket, void* ext_stream) override {
-#if !defined(ZKB_EMU)
-    ProofSlot& sl = slot_of(ticket);
-    Stream ext; ext.s = (cudaStream_t)ext_stream;
-    sl.ev_chains_done.wait(ext);
-#else
-    ProofSlot& sl = slot_of(ticket);
-    Stream ext; ext.s = (int)(intptr_t)ext_stream;   // an emulated stream (zkb_emu_stream_create)
-    sl.ev_chains_done.wait(ext);
-#endif
+    slot_of(ticket).ev_chains_done.wait(stream_from_handle(ext_stream));
   }
   void prove_stream_to_finish(uint64_t ticket, void* ext_stream) override {
-#if !defined(ZKB_EMU)
     ProofSlot& sl = slot_of(ticket);
-    Stream ext; ext.s = (cudaStream_t)ext_stream;
     if (!has_wm_stream_) throw Error(ZKB_E_INTERNAL, "no witness-map stream");
-    sl.ev_exchange.record(ext);
+    sl.ev_exchange.record(stream_from_handle(ext_stream));
     sl.ev_exchange.wait(wm_stream_);
-#else
-    ProofSlot& sl = slot_of(ticket);
-    Stream ext; ext.s = (int)(intptr_t)ext_stream;
-    if (!has_wm_stream_) throw Error(ZKB_E_INTERNAL, "no witness-map stream");
-    sl.ev_exchange.record(ext);
-    sl.ev_exchange.wait(wm_stream_);
-#endif
   }
   void prove_end_async(uint64_t ticket) override {
     ProofSlot& sl = slot_of(ticket);
@@ -2246,14 +2152,10 @@ class Engine : public EngineBase {
     if (opts.batch_pass_max > 0) kmax = std::min<uint64_t>(kmax, (uint64_t)opts.batch_pass_max);
     kmax = std::min<uint64_t>(kmax, K);
     if (kmax == 0) throw Error(ZKB_E_ARG, "msm too large");
-#if !defined(ZKB_EMU)
-    size_t free_b = 0, total_b = 0;
-    ZKB_CUDA(cudaMemGetInfo(&free_b, &total_b));
-    const size_t reserve = (size_t)1 << 30, have = free_b + batch_.device_bytes();
-    const size_t avail = have > reserve ? have - reserve : 0;
+    const size_t have = dev_mem_free() + batch_.device_bytes();
+    const size_t avail = have > DEV_MEM_RESERVE ? have - DEV_MEM_RESERVE : 0;
     for (size_t need = batch_bytes(pk, rc, kmax, pre_c_z, extra); kmax > 1 && need > avail; need = batch_bytes(pk, rc, kmax, pre_c_z, extra))
       kmax = std::max<uint64_t>(1, std::min<uint64_t>(kmax - 1, (uint64_t)((double)kmax * avail / need)));
-#endif
     return (uint32_t)kmax;
   }
 

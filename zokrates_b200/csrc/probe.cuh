@@ -71,10 +71,7 @@ static __global__ void zkb_probe_modmul(uint32_t iters, uint32_t seed, F* sink) 
 inline double peak_probe(Stream st, int kind, uint32_t iters) {
 #if !defined(ZKB_EMU)
   typedef Fp<Bn254Fq> F;
-  int dev = 0, sms = 0;
-  ZKB_CUDA(cudaGetDevice(&dev));
-  ZKB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-  const int block = 256, blocks = sms * 8;
+  const int block = 256, blocks = device_sm_count() * 8;
   DevBuf<uint64_t> sink(16);
   cudaEvent_t a, b;
   ZKB_CUDA(cudaEventCreate(&a));

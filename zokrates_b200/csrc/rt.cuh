@@ -1,4 +1,4 @@
-// Thin runtime layer: device memory, copies and kernel launches.
+// Thin runtime layer: devices, device memory, streams, copies, kernel launches and stage timers.
 //
 // Product build (nvcc, sm_90a): every `launch<Tag>(n, fn)` is a real kernel on the engine's CUDA
 // stream; failures surface as zkb::Error (never a silent CPU path).
@@ -12,10 +12,13 @@
 #include <string.h>
 #include <stdexcept>
 #include <string>
+#include <utility>
+#include <vector>
 #include "hd.cuh"
 #include "zkb.h"  // status codes (include/zkb.h)
 
 #if !defined(ZKB_EMU)
+#include <atomic>
 #include <cuda_runtime.h>
 #else
 #include <deque>
@@ -24,7 +27,6 @@
 #include <memory>
 #include <mutex>
 #include <set>
-#include <vector>
 #endif
 
 namespace zkb {
@@ -69,24 +71,6 @@ inline void launch(Stream st, size_t n, Fn fn) {
   size_t blocks = (n + BLOCK - 1) / BLOCK;
   if (blocks > 0x7fffffffull) throw Error(ZKB_E_ARG, "grid too large");
   zkb_kernel<Tag, BLOCK, MINB, Fn><<<(unsigned)blocks, BLOCK, 0, st.s>>>(n, fn);
-  ZKB_CUDA(cudaGetLastError());
-}
-
-// Block-cooperative kernels: `nphases` steps separated by __syncthreads(); threads of a block exchange data
-// through (L1-coherent) global scratch.  fn(block, thread, phase).  The host emulation runs phase by phase.
-template <class Tag, int BLOCK, class Fn>
-__global__ void __launch_bounds__(BLOCK) zkb_phased_kernel(uint32_t nphases, Fn fn) {
-  for (uint32_t ph = 0; ph < nphases; ph++) {
-    fn((uint32_t)blockIdx.x, (uint32_t)threadIdx.x, ph);
-    __syncthreads();
-  }
-}
-template <class Tag, int BLOCK, class Fn>
-inline void launch_phased(Stream st, size_t nblocks, uint32_t nphases, Fn fn) {
-  if (nblocks == 0) return;
-  launch_counter()++;
-  if (nblocks > 0x7fffffffull) throw Error(ZKB_E_ARG, "grid too large");
-  zkb_phased_kernel<Tag, BLOCK, Fn><<<(unsigned)nblocks, BLOCK, 0, st.s>>>(nphases, fn);
   ZKB_CUDA(cudaGetLastError());
 }
 
@@ -158,6 +142,50 @@ struct Event {
   void sync() { if (e) ZKB_CUDA(cudaEventSynchronize(e)); }     // host waits
   void destroy() { if (e) { cudaEventDestroy(e); e = nullptr; } }
 };
+// stage timer: named spans between CUDA events on a stream (no-op in the host emulation)
+struct StageTimer {
+  struct Ev { const char* name; cudaEvent_t a, b; };
+  std::vector<Ev> evs;
+  std::vector<size_t> open;  // stack of stages begun but not ended (stages may nest)
+  Stream st;
+  explicit StageTimer(Stream s) : st(s) {}
+  void begin(const char* name) {
+    Ev e{name, nullptr, nullptr};
+    ZKB_CUDA(cudaEventCreate(&e.a));
+    ZKB_CUDA(cudaEventCreate(&e.b));
+    ZKB_CUDA(cudaEventRecord(e.a, st.s));
+    open.push_back(evs.size());
+    evs.push_back(e);
+  }
+  void end() {
+    size_t i = open.back();
+    open.pop_back();
+    ZKB_CUDA(cudaEventRecord(evs[i].b, st.s));
+  }
+  // spans on other streams (tails): begin_on returns a handle for end_on
+  size_t begin_on(Stream s, const char* name) {
+    Ev e{name, nullptr, nullptr};
+    ZKB_CUDA(cudaEventCreate(&e.a));
+    ZKB_CUDA(cudaEventCreate(&e.b));
+    ZKB_CUDA(cudaEventRecord(e.a, s.s));
+    evs.push_back(e);
+    return evs.size() - 1;
+  }
+  void end_on(Stream s, size_t i) { ZKB_CUDA(cudaEventRecord(evs[i].b, s.s)); }
+  void collect(std::vector<std::pair<const char*, double>>& out) {
+    out.clear();
+    for (auto& e : evs) {
+      ZKB_CUDA(cudaEventSynchronize(e.b));
+      float ms = 0;
+      ZKB_CUDA(cudaEventElapsedTime(&ms, e.a, e.b));
+      out.push_back({e.name, (double)ms});
+      cudaEventDestroy(e.a);
+      cudaEventDestroy(e.b);
+    }
+    evs.clear();
+  }
+  ~StageTimer() { for (auto& e : evs) { cudaEventDestroy(e.a); cudaEventDestroy(e.b); } }
+};
 // page-locked host memory (asynchronous device -> host copies land here while the next proof's kernels run)
 inline void* host_alloc_pinned(size_t bytes) {
   void* p = nullptr;
@@ -165,6 +193,48 @@ inline void* host_alloc_pinned(size_t bytes) {
   return p;
 }
 inline void host_free_pinned(void* p) { if (p) cudaFreeHost(p); }
+
+// ---- devices -------------------------------------------------------------------------------------------------------------
+inline size_t dev_mem_free() {
+  size_t free_b = 0, total_b = 0;
+  ZKB_CUDA(cudaMemGetInfo(&free_b, &total_b));
+  return free_b;
+}
+// multiprocessor count of the current device, queried once per device
+inline int device_sm_count() {
+  static std::atomic<int> cached[64];
+  int dev = 0, n = 0;
+  ZKB_CUDA(cudaGetDevice(&dev));
+  if (dev < 64) n = cached[dev].load(std::memory_order_relaxed);
+  if (!n) {
+    ZKB_CUDA(cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev));
+    if (dev < 64) cached[dev].store(n, std::memory_order_relaxed);
+  }
+  return n;
+}
+// visible devices, or -1 with *why set to the reason (the failed query is not left as the thread's last error)
+inline int device_count(const char** why) {
+  int n = 0;
+  const cudaError_t e = cudaGetDeviceCount(&n);
+  if (e == cudaSuccess) return n;
+  cudaGetLastError();
+  *why = cudaGetErrorString(e);
+  return -1;
+}
+inline void device_select(int dev) { ZKB_CUDA(cudaSetDevice(dev)); }
+// a failed launch configuration sticks as the thread's last error; clear it before the next call checks its own launches
+inline void clear_device_error() { cudaGetLastError(); }
+// before a context's engine is destroyed: wait for the context's main stream on its device; never throws (zkb_ctx_destroy)
+inline void device_drain(int dev, Stream st) {
+  cudaSetDevice(dev);
+  if (st.s) cudaStreamSynchronize(st.s);
+}
+// a caller's stream passed through the C ABI as void* (cudaStream_t)
+inline Stream stream_from_handle(void* h) {
+  Stream s;
+  s.s = (cudaStream_t)h;
+  return s;
+}
 
 #else  // ------------------------------------------------------------------ host emulation (tests)
 
@@ -386,22 +456,6 @@ inline void launch(Stream st, size_t n, Fn fn) {
   });
 }
 // Phases stay in sequence (each stands for a __syncthreads()); blocks, and threads within a phase, are permuted.
-template <class Tag, int BLOCK, class Fn>
-inline void launch_phased(Stream st, size_t nblocks, uint32_t nphases, Fn fn) {
-  if (!nblocks) return;
-  const uint64_t id = ++launch_counter();
-  const EmuOrder o = emu_order();
-  emu_enqueue(st, [=] {
-    EmuPerm bperm(nblocks, id, o);
-    for (size_t i = 0; i < nblocks; i++) {
-      uint32_t b = (uint32_t)bperm(i);
-      for (uint32_t ph = 0; ph < nphases; ph++) {
-        EmuPerm tperm(BLOCK, emu_mix(id) ^ ((uint64_t)b << 20) ^ ph, o);
-        for (uint32_t t = 0; t < (uint32_t)BLOCK; t++) fn(b, (uint32_t)tperm(t), ph);
-      }
-    }
-  });
-}
 template <class Tag, int BLOCK, int SMEM_BYTES, class Fn>
 inline void launch_block(Stream st, size_t nblocks, uint32_t nphases, Fn fn) {
   if (!nblocks) return;
@@ -491,6 +545,14 @@ struct Event {
   }
   void destroy() { sid = -1; }
 };
+struct StageTimer {
+  explicit StageTimer(Stream) {}
+  void begin(const char*) {}
+  void end() {}
+  size_t begin_on(Stream, const char*) { return 0; }
+  void end_on(Stream, size_t) {}
+  void collect(std::vector<std::pair<const char*, double>>& out) { out.clear(); }
+};
 inline void* host_alloc_pinned(size_t bytes) {
   if (bytes == 0) bytes = 16;
   void* p = malloc(bytes);
@@ -512,7 +574,26 @@ inline void host_free_pinned(void* p) {
   free(p);
 }
 
+// ---- one emulated device ------------------------------------------------------------------------------------------------
+// Half the address space, so every memory clamp runs and none binds: a pass size derived from it is far above any batch,
+// and adding the device bytes a caller already holds cannot overflow.  Pass sizes come from the other limits alone.
+inline size_t dev_mem_free() { return ~(size_t)0 >> 1; }
+inline int device_sm_count() { return 1; }   // read only by device-only launches (the tile2 NTT)
+inline int device_count(const char**) { return 1; }
+inline void device_select(int) {}
+inline void clear_device_error() {}
+// runs the work queued on every stream, not only the context's, as the engine's first dev_free would
+inline void device_drain(int, Stream) { emu_drain_all(); }
+inline Stream stream_from_handle(void* h) {   // an emulated stream id (zkb_emu_stream_create)
+  Stream s;
+  s.s = (int)(intptr_t)h;
+  return s;
+}
+
 #endif
+
+// free device memory every pass-size and window-table budget leaves unused
+static constexpr size_t DEV_MEM_RESERVE = (size_t)1 << 30;
 
 // RAII device buffer
 template <class T>
